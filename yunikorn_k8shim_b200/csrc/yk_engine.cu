@@ -275,6 +275,7 @@ struct yk_engine {
     bool un_alloc = false, un_ord_stale = false;   // un_ord_stale: uniform runs moved nodes since d_ord was last written
     const uint32_t* lt_shape_ids = nullptr;     // per ask: a number equal for equal request vectors (a_shape, or a_sigid: finer, still exact)
     int un_min = 2048;                          // shortest run that takes the uniform path (YK_UNIFORM_MIN)
+    int un_depth = 0;                           // first depth of a uniform run's attempt (YK_UNIFORM_DEPTH); 0: ykun::first_depth
     Dev<unsigned long long> d_un_ekey[2], d_un_bk, d_un_rkey[2], d_un_rrn[2];
     Dev<uint32_t> d_un_enode[2], d_un_cnt;
     Dev<ykun::Globals> d_un_g; Pin<ykun::Globals> h_un_g;
@@ -571,6 +572,7 @@ int lt_uniform(yk_engine* e, size_t off, size_t R, bool insensitive, bool has_ga
         for (int k = 0; k < e->D; ++k) if (e->w.w[k] != 0.0 && a.req[k] != 0) flat = false;
         if (flat) L = Lmax;
     }
+    if (e->un_depth > 0) L = e->un_depth;   // testing knob: a shallow first attempt makes the retry path reachable
     L = std::min(L, Lmax);
     for (;;) {
         if ((size_t)L * (size_t)nlive > UN_EMAX) return YK_OK;   // too deep for the element buffers: fallback
@@ -1166,6 +1168,7 @@ int yk_create(const yk_config* cfg, yk_engine** out) {
     e->lt_prof = getenv("YK_PROFILE_LATTICE") != nullptr;
     e->hp_on = getenv("YK_PROFILE_HOST") != nullptr;
     if (const char* um = getenv("YK_UNIFORM_MIN")) e->un_min = atoi(um);   // 0: no uniform-run path
+    if (const char* ud = getenv("YK_UNIFORM_DEPTH")) e->un_depth = std::max(0, atoi(ud));   // 0 / unset: the engine's own rule
     T(e->d_lt_prof.alloc(16));
     if (ok) T(cudaMemset(e->d_lt_prof.p, 0, 16 * sizeof(long long)));
     if (ok) T(lattice_setup(D, &e->lt_smem));
@@ -1545,9 +1548,13 @@ int run_lattice(yk_engine* e, Cycle& c, bool& handoff) {
                 while (consumed < B && e->cm.same_gang(A.asks[0], A.asks[consumed])) ++consumed;
             if (!ins) status = yklt::ST_STOPPED;
         } else {
+            if (first) {   // the initial order's NaN flag (device_order) is checked before the first batch commits anything:
+                           // a failed cycle must leave the node tables as they were
+                CK(cudaStreamSynchronize(e->stream));
+                if (e->h_flag[0]) return e->fail(YK_ERR_RANGE, "NaN node score (zero total on a weighted resource)");
+            }
             rc = lt_batch(e, B, ins);
             if (rc) return rc;
-            if (first && e->h_flag[0]) return e->fail(YK_ERR_RANGE, "NaN node score (zero total on a weighted resource)");
             status = e->h_lt_hdr[yklt::H_STATUS];
             consumed = (size_t)e->h_lt_hdr[yklt::H_CONSUMED];
             if (status == yklt::ST_NAN) return e->fail(YK_ERR_RANGE, "NaN node score after commit");

@@ -593,3 +593,18 @@ def redim(s: Snapshot, D2: int, seed: int = 0) -> Snapshot:
     s.weights, s.D = w, D2
     s.name = f"{s.name}-D{D2}"
     return s
+
+
+def reweigh(s: Snapshot, w) -> Snapshot:
+    """The same snapshot with node-sort weights `w` (one per resource dimension, >= 0) -- the scheduler's configured
+    resource weights instead of the default vcore = memory = 1."""
+    import copy
+    w = np.asarray(w, dtype=np.float64)
+    if w.shape != (s.D,):
+        raise ValueError(f"expected {s.D} weights, got shape {w.shape}")
+    if (w < 0).any() or not np.isfinite(w).all():
+        raise ValueError("weights must be finite and >= 0")
+    s = copy.deepcopy(s)
+    s.weights = w.copy()
+    s.name = f"{s.name}-w{'_'.join(f'{x:g}' for x in w)}"
+    return s

@@ -80,6 +80,7 @@ type askRec struct {
 	node      uint32 // foreign / recovered: the node it sits on
 	lastState uint8  // last state reported through UpdateContainerSchedulingState
 	slow      bool
+	exact     bool // slow only for needsGoPredicates: the dictionary encoded the pod's masks exactly (yk_filter_nodes applies)
 	present   bool
 }
 
@@ -577,13 +578,13 @@ func needsGoPredicates(p *v1.Pod) bool {
 	return len(p.Spec.TopologySpreadConstraints) > 0
 }
 
-// podMasks: nodeSelector + required node affinity + tolerations + spec.nodeName -> yk_pod_masks
-func (e *Engine) podMasks(p *v1.Pod) C.yk_pod_masks {
-	var out C.yk_pod_masks
+// podMasks: nodeSelector + required node affinity + tolerations + spec.nodeName -> yk_pod_masks.  exact: the dictionary
+// encoded all of them (it did not set YK_ASK_SLOWPATH itself; needsGoPredicates may still have)
+func (e *Engine) podMasks(p *v1.Pod) (out C.yk_pod_masks, exact bool) {
 	out.required_node = C.YK_NONE
 	if p == nil {
 		out.flags = C.YK_ASK_SLOWPATH
-		return out
+		return out, false
 	}
 	var held []unsafe.Pointer
 	hold := func(s string) *C.char { c := C.CString(s); held = append(held, unsafe.Pointer(c)); return c }
@@ -658,10 +659,11 @@ func (e *Engine) podMasks(p *v1.Pod) C.yk_pod_masks {
 		spec.node_name = hold(p.Spec.NodeName)
 	}
 	C.yk_dict_pod(e.dict, &spec, &out)
+	exact = out.flags&C.YK_ASK_SLOWPATH == 0
 	if needsGoPredicates(p) {
 		out.flags |= C.YK_ASK_SLOWPATH
 	}
-	return out
+	return out, exact
 }
 
 // dictionary handed out new bits while compiling a pod: node bit sets (and key-only tolerations) were extended
@@ -713,8 +715,9 @@ func (e *Engine) pushAsk(idx uint32, a *askRec, alloc *si.Allocation) error {
 	if e.src != nil {
 		pod = e.src.GetPod(a.key)
 	}
-	m := e.podMasks(pod)
+	m, exact := e.podMasks(pod)
 	a.slow = m.flags&C.YK_ASK_SLOWPATH != 0
+	a.exact = exact
 	app, ok := e.appIdx[a.app]
 	if !ok {
 		return fmt.Errorf("ask %s: unknown application %s", a.key, a.app)
@@ -896,6 +899,22 @@ func (e *Engine) collectStates() []*si.UpdateContainerSchedulingStateRequest {
 	if C.yk_ask_states(e.h, C.uint32_t(len(idx)), &idx[0], &st[0]) != C.YK_OK {
 		return nil
 	}
+	// the asks newly NOFIT get a per-cause reason, from one yk_filter_nodes call over all of them
+	var nofit []C.uint32_t
+	for j, i := range idx {
+		if s := uint8(st[j]); s == C.YK_ST_NOFIT && s != e.asks[i].lastState {
+			nofit = append(nofit, i)
+		}
+	}
+	reason := map[C.uint32_t]string{}
+	if len(nofit) > 0 {
+		counts := make([]C.uint32_t, len(nofit)*C.YK_FILTER_SLOTS)
+		if C.yk_filter_nodes(e.h, C.uint32_t(len(nofit)), &nofit[0], 1, 0, 0, nil, nil, &counts[0]) == C.YK_OK {
+			for j, i := range nofit {
+				reason[i] = failedReason(counts[j*C.YK_FILTER_SLOTS : (j+1)*C.YK_FILTER_SLOTS])
+			}
+		}
+	}
 	var out []*si.UpdateContainerSchedulingStateRequest
 	for j, i := range idx {
 		a := &e.asks[i]
@@ -906,8 +925,12 @@ func (e *Engine) collectStates() []*si.UpdateContainerSchedulingStateRequest {
 		a.lastState = s
 		switch s {
 		case C.YK_ST_NOFIT:
+			r, ok := reason[i]
+			if !ok {
+				r = "no node passes the predicates with enough resources"
+			}
 			out = append(out, &si.UpdateContainerSchedulingStateRequest{ApplicationID: a.app, AllocationKey: a.key,
-				State: si.UpdateContainerSchedulingStateRequest_FAILED, Reason: "no node passes the predicates with enough resources"})
+				State: si.UpdateContainerSchedulingStateRequest_FAILED, Reason: r})
 		case C.YK_ST_SKIPPED:
 			out = append(out, &si.UpdateContainerSchedulingStateRequest{ApplicationID: a.app, AllocationKey: a.key,
 				State: si.UpdateContainerSchedulingStateRequest_SKIPPED, Reason: "request exceeds the queue headroom"})
@@ -916,74 +939,195 @@ func (e *Engine) collectStates() []*si.UpdateContainerSchedulingStateRequest {
 	return out
 }
 
+// failedReason: the FAILED reason of an unplaceable pod in the Kubernetes scheduler's style, from the yk_filter_nodes
+// counts of its ask (one count per first failing step, summing to the node count), e.g.
+// "0/5000 nodes are available: 3 node(s) were unschedulable, 4990 Insufficient resources, 7 node(s) had untolerated taint."
+// Steps with no node are left out; a node too small (total), too full (available) or failing NodeResourcesFit counts as
+// "Insufficient resources".
+func failedReason(c []C.uint32_t) string {
+	total := uint64(0)
+	for _, x := range c {
+		total += uint64(x)
+	}
+	parts := make([]string, 0, 8)
+	add := func(n uint64, text string) {
+		if n > 0 {
+			parts = append(parts, fmt.Sprintf("%d %s", n, text))
+		}
+	}
+	add(uint64(c[C.YK_FAIL_NODE_NOT_SCHEDULABLE]), "node(s) were unschedulable")
+	add(uint64(c[C.YK_FAIL_TOTAL])+uint64(c[C.YK_FAIL_AVAILABLE])+uint64(c[C.YK_FAIL_RESOURCES]), "Insufficient resources")
+	add(uint64(c[C.YK_FAIL_REQUEST_NOT_POSITIVE]), "request not positive")
+	add(uint64(c[C.YK_FAIL_NODENAME]), "node(s) didn't match the requested node name")
+	add(uint64(c[C.YK_FAIL_TAINT]), "node(s) had untolerated taint")
+	add(uint64(c[C.YK_FAIL_AFFINITY]), "node(s) didn't match Pod's node affinity/selector")
+	add(uint64(c[C.YK_FAIL_ABSENT]), "node(s) not found")
+	add(uint64(c[C.YK_FILTER_RESERVED]), "node(s) were reserved")
+	return fmt.Sprintf("0/%d nodes are available: %s.", total, strings.Join(parts, ", "))
+}
+
+// filterPage: one page of the engine's candidates for ask idx -- the nodes that pass every step the engine checks, in its
+// node order, pass ranks skip .. skip+filterPageSize-1 -- as node names, and how many nodes pass in all.  Caller holds e.mu.
+const filterPageSize = 64
+
+func (e *Engine) filterPage(idx uint32, skip uint32) ([]string, uint32, bool) {
+	page := make([]C.uint32_t, filterPageSize)
+	var npass C.uint32_t
+	i := C.uint32_t(idx)
+	if C.yk_filter_nodes(e.h, 1, &i, 1, C.uint32_t(skip), filterPageSize, &page[0], &npass, nil) != C.YK_OK {
+		return nil, 0, false
+	}
+	return e.pageNames(page), uint32(npass), true
+}
+
+func (e *Engine) pageNames(page []C.uint32_t) []string {
+	names := make([]string, 0, len(page))
+	for _, x := range page {
+		if x == C.YK_NONE {
+			break
+		}
+		names = append(names, e.nodes[x].name)
+	}
+	return names
+}
+
 // slowPath: pods whose predicates do not reduce to the bit sets.  Candidates are tried in the engine's node order
 // (ascending float64 score, then NodeID) through the UNCHANGED Go path -- callback.Predicates ->
 // Context.IsPodFitNode -> PredicateManager (scheduler_callback.go:196-198) -- and the first node that passes is pinned:
 // the ask goes back to the engine naming that node (spec.nodeName semantics), everything else tolerated, so the next
 // cycle re-checks the resources, commits and reports the binding like any other.
+// An ask whose masks the dictionary encoded exactly (slow only for what needsGoPredicates names) walks only the nodes that
+// pass the engine's own steps, a page of yk_filter_nodes at a time: every engine step is also a step of the
+// PredicateManager (or of the core before it), so a node skipped there could never pass, and in the same order the first
+// Go-passing candidate is the node the full walk reaches.  Every other slow-path ask walks every live node.
 func (e *Engine) slowPath(cb api.ResourceManagerCallback, askIdxs []uint32) {
 	if len(askIdxs) == 0 {
 		return
 	}
 	e.mu.Lock()
-	live := make([]uint32, 0, len(e.nodes))
-	for i := range e.nodes {
-		if e.nodes[i].present && e.nodes[i].schedulable {
-			live = append(live, uint32(i))
-		}
-	}
-	ci := make([]C.uint32_t, len(live))
-	for i, x := range live {
-		ci[i] = C.uint32_t(x)
-	}
-	scores := make([]C.double, len(live))
-	if len(live) > 0 {
-		C.yk_node_scores(e.h, C.uint32_t(len(live)), &ci[0], &scores[0])
-	}
-	sort.Slice(live, func(a, b int) bool {
-		if scores[a] != scores[b] {
-			return scores[a] < scores[b]
-		}
-		return e.nodes[live[a]].name < e.nodes[live[b]].name
-	})
-	names := make([]string, len(live))
-	for i, x := range live {
-		names[i] = e.nodes[x].name
-	}
 	type job struct {
-		idx uint32
-		key string
+		idx   uint32
+		key   string
+		exact bool
+		page  []string // first page of candidates (exact asks)
+		npass uint32
 	}
 	jobs := make([]job, 0, len(askIdxs))
+	var exactIdx []C.uint32_t
 	for _, a := range askIdxs {
 		if int(a) < len(e.asks) && e.asks[a].present {
-			jobs = append(jobs, job{a, e.asks[a].key})
+			jobs = append(jobs, job{idx: a, key: e.asks[a].key, exact: e.asks[a].exact})
+			if e.asks[a].exact {
+				exactIdx = append(exactIdx, C.uint32_t(a))
+			}
+		}
+	}
+	// the first page of every exact ask in one call; if it fails they walk every node like the others
+	if len(exactIdx) > 0 {
+		first := make([]C.uint32_t, len(exactIdx)*filterPageSize)
+		npass := make([]C.uint32_t, len(exactIdx))
+		ok := C.yk_filter_nodes(e.h, C.uint32_t(len(exactIdx)), &exactIdx[0], 1, 0, filterPageSize, &first[0], &npass[0], nil) == C.YK_OK
+		x := 0
+		for j := range jobs {
+			if !jobs[j].exact {
+				continue
+			}
+			if ok {
+				jobs[j].page = e.pageNames(first[x*filterPageSize : (x+1)*filterPageSize])
+				jobs[j].npass = uint32(npass[x])
+			} else {
+				jobs[j].exact = false
+			}
+			x++
+		}
+	}
+	walkAll := false
+	for _, j := range jobs {
+		walkAll = walkAll || !j.exact
+	}
+	var names []string // every live node in the engine's order, for the asks that walk them all
+	if walkAll {
+		live := make([]uint32, 0, len(e.nodes))
+		for i := range e.nodes {
+			if e.nodes[i].present && e.nodes[i].schedulable {
+				live = append(live, uint32(i))
+			}
+		}
+		ci := make([]C.uint32_t, len(live))
+		for i, x := range live {
+			ci[i] = C.uint32_t(x)
+		}
+		scores := make([]C.double, len(live))
+		if len(live) > 0 {
+			C.yk_node_scores(e.h, C.uint32_t(len(live)), &ci[0], &scores[0])
+		}
+		sort.Slice(live, func(a, b int) bool {
+			if scores[a] != scores[b] {
+				return scores[a] < scores[b]
+			}
+			return e.nodes[live[a]].name < e.nodes[live[b]].name
+		})
+		names = make([]string, len(live))
+		for i, x := range live {
+			names[i] = e.nodes[x].name
 		}
 	}
 	e.mu.Unlock()
 	for _, j := range jobs {
 		chosen := ""
-		for _, node := range names {
-			if cb.Predicates(&si.PredicatesArgs{AllocationKey: j.key, NodeID: node, Allocate: true}) == nil {
-				chosen = node
-				break
+		if j.exact {
+			chosen = e.walkCandidates(cb, j.idx, j.key, j.page, j.npass)
+		} else {
+			for _, node := range names {
+				if cb.Predicates(&si.PredicatesArgs{AllocationKey: j.key, NodeID: node, Allocate: true}) == nil {
+					chosen = node
+					break
+				}
 			}
 		}
-		e.mu.Lock()
-		a := &e.asks[j.idx]
-		if chosen == "" || !a.present || a.key != j.key {
-			e.mu.Unlock()
-			continue // no node passes today: the ask stays SLOWPATH and is tried again next cycle
-		}
-		i, rn, all, zero, fl := C.uint32_t(j.idx), C.uint32_t(e.nodeIdx[chosen]), ^C.uint64_t(0), C.uint64_t(0), C.uint32_t(0)
-		var rq [4]C.int64_t
-		for k := 0; k < 4; k++ {
-			rq[k] = C.int64_t(a.req[k])
-		}
-		app := C.uint32_t(e.appIdx[a.app])
-		prio, seq := C.int32_t(0), C.int64_t(0) // first in its application: it was reached in order already
-		C.yk_asks_upsert(e.h, 1, &i, &rq[0], &all, &zero, &zero, &prio, &seq, &app, &rn, &fl, nil)
-		e.mu.Unlock()
-		e.wake()
+		e.pinSlowAsk(j.idx, j.key, chosen)
 	}
+}
+
+// walkCandidates: the first of the engine's candidates for an exact slow-path ask that the Go predicates accept, page by
+// page (the first page is given), until one passes or the candidates run out; "" when none does
+func (e *Engine) walkCandidates(cb api.ResourceManagerCallback, idx uint32, key string, page []string, npass uint32) string {
+	for skip := uint32(0); ; {
+		for _, node := range page {
+			if cb.Predicates(&si.PredicatesArgs{AllocationKey: key, NodeID: node, Allocate: true}) == nil {
+				return node
+			}
+		}
+		skip += filterPageSize
+		if skip >= npass {
+			return ""
+		}
+		e.mu.Lock()
+		var ok bool
+		page, npass, ok = e.filterPage(idx, skip)
+		e.mu.Unlock()
+		if !ok {
+			return ""
+		}
+	}
+}
+
+// pinSlowAsk: the chosen node goes back to the engine as the ask's node name; "" leaves the ask as it is
+func (e *Engine) pinSlowAsk(idx uint32, key, chosen string) {
+	e.mu.Lock()
+	a := &e.asks[idx]
+	if chosen == "" || !a.present || a.key != key {
+		e.mu.Unlock()
+		return // no node passes today: the ask stays SLOWPATH and is tried again next cycle
+	}
+	i, rn, all, zero, fl := C.uint32_t(idx), C.uint32_t(e.nodeIdx[chosen]), ^C.uint64_t(0), C.uint64_t(0), C.uint32_t(0)
+	var rq [4]C.int64_t
+	for k := 0; k < 4; k++ {
+		rq[k] = C.int64_t(a.req[k])
+	}
+	app := C.uint32_t(e.appIdx[a.app])
+	prio, seq := C.int32_t(0), C.int64_t(0) // first in its application: it was reached in order already
+	C.yk_asks_upsert(e.h, 1, &i, &rq[0], &all, &zero, &zero, &prio, &seq, &app, &rn, &fl, nil)
+	e.mu.Unlock()
+	e.wake()
 }

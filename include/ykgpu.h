@@ -30,6 +30,9 @@
  *                                       (pkg/cache/scheduler_callback.go:218-222, context.go:1232-1272)
  *   yk_evaluate                         one ResourceManagerCallback.Predicates(ask,node) answer, for the
  *                                       slow-path bridge and for known-answer tests
+ *   yk_filter_nodes                     the same answers for every node and a list of asks at once: the candidates a
+ *                                       slow-path pod is walked through Predicates in, and the per-cause counts of the
+ *                                       FAILED reason of an unplaceable pod
  *
  * Conventions: every call returns YK_OK (0) or a negative yk_status; no exceptions or aborts cross the
  * boundary.  Inputs are caller-owned host memory, fully consumed before return (cgo: no Go pointer is
@@ -235,6 +238,30 @@ int yk_evaluate(yk_engine* e, uint32_t ask, uint32_t node);
 int yk_evaluate_reserve(yk_engine* e, uint32_t ask, uint32_t node);
 /* node sort keys as the device computes them (float64 score bits), for known-answer tests */
 int yk_node_scores(yk_engine* e, uint32_t n, const uint32_t* idx, double* score_out);
+
+/* Every present node's first failing step for a list of asks, in the cycle's node order, evaluated on the device in one
+ * grid-wide pass (csrc/yk_filter.cuh).  For the slow-path bridge (walk only the nodes that pass the engine's own steps, in
+ * the engine's order, through the Go PredicateManager) and for the per-cause FAILED reason of an unplaceable pod.  Read-only.
+ *   Nodes considered: every present node, ordered exactly as yk_cycle would order them now -- ascending float64 score under
+ *     the engine's policy and weights (yk_score.h), ties by name_rank, then by node index.
+ *   Slot of a pair: YK_FILTER_RESERVED if the node is flagged YK_NODE_RESERVED (hidden from the core's node iterator, never
+ *     evaluated); otherwise exactly what yk_evaluate(ask, node) returns -- yk_evaluate_reserve(ask, node) when allocate == 0 --
+ *     on the current tables; slot 0 = passes.  An ask that is not present counts every node in slot YK_FAIL_ABSENT and has
+ *     no candidates.  counts[i*YK_FILTER_SLOTS + slot] (may be NULL) sums to the number of present nodes.
+ *   Candidates: nodes_out[i*k + j] = the passing node of rank skip + j in that order (j < k), YK_NONE past the last one;
+ *     n_pass[i] (may be NULL) = the number of passing nodes = counts[i*YK_FILTER_SLOTS].  With allocate == 1 and no reserved
+ *     node, candidate 0 (skip = 0) is the node the frozen-snapshot sweep of a cycle picks for that ask.
+ *   Node side only: queue headroom, user limits, gangs and YK_ASK_SLOWPATH play no part, as in yk_evaluate.
+ *   Errors: YK_ERR_ARG for an ask index >= max_asks, k > 0 with nodes_out == NULL, or n > 0 with asks == NULL;
+ *     YK_ERR_RANGE when a present node scores NaN (as yk_cycle), and then nothing is written.  n == 0 is YK_OK.
+ *   No state changes: stale tables are uploaded and the nodes sorted in the filter's own device buffers, so the next yk_cycle
+ *     is the same whether or not this ran.  Counted in other_launches / h2d_bytes / d2h_bytes; local to this engine
+ *     whatever rank / world are. */
+#define YK_FILTER_SLOTS 11      /* slot 0 = passes, 1..9 = the YK_FAIL_* answer of yk_evaluate, 10 = reserved */
+#define YK_FILTER_RESERVED 10   /* YK_NODE_RESERVED: hidden from the core's node iterator, never evaluated */
+int yk_filter_nodes(yk_engine* e, uint32_t n, const uint32_t* asks, int allocate, uint32_t skip, uint32_t k,
+                    uint32_t* nodes_out /* [n][k] row-major, YK_NONE padded, may be NULL iff k == 0 */,
+                    uint32_t* n_pass /* [n], may be NULL */, uint32_t* counts /* [n][YK_FILTER_SLOTS] row-major, may be NULL */);
 
 /* Preemption victim search, batched (ResourceManagerCallback.PreemptionPredicates,
  * pkg/cache/scheduler_callback.go:200-209 -> context.go:705-729 -> predicate_manager.go:137-175).  Query q: the

@@ -27,6 +27,7 @@
 #include <x86intrin.h>
 
 #include "yk_kernels.cuh"
+#include "yk_filter.cuh"
 #include "yk_lattice.cuh"
 #include "yk_uniform.cuh"
 #include "yk_commit.hpp"
@@ -282,6 +283,11 @@ struct yk_engine {
     Dev<uint8_t> d_un_cub; size_t un_cub_bytes = 0;
     std::vector<ykun::Segment> un_segs;
     Dev<uint32_t> pre_q; Dev<int64_t> pre_v; Dev<int32_t> pre_o;   // yk_preemption_search staging, grown on demand
+    // yk_filter_nodes: its own node order (so a cycle's sort buffers are never touched) and per-chunk buffers, grown on demand
+    Dev<uint64_t> f_key_in, f_key_out; Dev<uint32_t> f_val_in, f_val_out; Dev<uint8_t> f_cub; size_t f_cub_bytes = 0;
+    Dev<int> f_flag; Pin<int> h_f_flag;
+    Dev<uint32_t> f_asks, f_bits, f_tcnt, f_counts, f_out;
+    Pin<uint32_t> h_f_asks, h_f_counts, h_f_out;
     yk_allgather_fn xfn = nullptr; void* xctx = nullptr;
     // peer-to-peer exchange (see yk_peer_export): peers' slot buffers and sync blocks, mapped through CUDA IPC
     bool p2p = false;
@@ -1899,6 +1905,32 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
     return rc ? rc : rc_end;
 }
 
+namespace {
+
+constexpr uint32_t FILTER_CHUNK = 4096;      // asks per yk_filter_kernel launch at most
+constexpr size_t FILTER_WORDS = 1u << 24;    // device words per chunk at most (bitmap + tile counts + counts + window)
+constexpr int FILTER_AC = 32;                // asks per shared-memory stage of yk_filter_kernel
+
+void launch_filter(int D, const YkFilterArgs& a, dim3 grid, cudaStream_t s) {
+    switch (D) {
+        case 1: yk_filter_kernel<1, FILTER_AC><<<grid, YK_FILTER_THREADS, 0, s>>>(a); break;
+        case 2: yk_filter_kernel<2, FILTER_AC><<<grid, YK_FILTER_THREADS, 0, s>>>(a); break;
+        case 3: yk_filter_kernel<3, FILTER_AC><<<grid, YK_FILTER_THREADS, 0, s>>>(a); break;
+        case 4: yk_filter_kernel<4, FILTER_AC><<<grid, YK_FILTER_THREADS, 0, s>>>(a); break;
+        case 5: yk_filter_kernel<5, FILTER_AC><<<grid, YK_FILTER_THREADS, 0, s>>>(a); break;
+        case 6: yk_filter_kernel<6, FILTER_AC><<<grid, YK_FILTER_THREADS, 0, s>>>(a); break;
+        case 7: yk_filter_kernel<7, FILTER_AC><<<grid, YK_FILTER_THREADS, 0, s>>>(a); break;
+        default: yk_filter_kernel<8, FILTER_AC><<<grid, YK_FILTER_THREADS, 0, s>>>(a); break;
+    }
+}
+
+template <typename T>
+cudaError_t grow(Dev<T>& d, size_t n) { return d.n < n ? d.alloc(n) : cudaSuccess; }
+template <typename T>
+cudaError_t grow(Pin<T>& h, size_t n) { return h.n < n ? h.alloc(n) : cudaSuccess; }
+
+}  // namespace
+
 extern "C" {
 
 int yk_ask_states(yk_engine* e, uint32_t n, const uint32_t* idx, uint8_t* out) {
@@ -2000,6 +2032,99 @@ int yk_preemption_search(yk_engine* e, uint32_t nq, const uint32_t* ask, const u
     CK(cudaMemcpyAsync(out, d_o.p, 4 * (size_t)nq, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     e->st.other_launches++;
+    return YK_OK;
+}
+
+int yk_filter_nodes(yk_engine* e, uint32_t n, const uint32_t* asks, int allocate, uint32_t skip, uint32_t k,
+                    uint32_t* nodes_out, uint32_t* n_pass, uint32_t* counts) {
+    if (!e) return YK_ERR_ARG;
+    std::lock_guard<std::mutex> g(e->mu);
+    if (n && !asks) return e->fail(YK_ERR_ARG, "yk_filter_nodes: null asks");
+    if (k && !nodes_out) return e->fail(YK_ERR_ARG, "yk_filter_nodes: null nodes_out with k > 0");
+    for (uint32_t i = 0; i < n; ++i) if (asks[i] >= e->maxA) return e->fail(YK_ERR_ARG, "yk_filter_nodes: ask index beyond max_asks");
+    if (!n) return YK_OK;
+    int rc = upload_tables(e);
+    if (rc) return rc;
+    const uint32_t nlive = e->nlive;
+    if (nlive == 0) {   // no node: nothing passes, nothing to count
+        if (k) std::fill(nodes_out, nodes_out + (size_t)n * k, YK_NONE);
+        if (n_pass) std::fill(n_pass, n_pass + n, 0u);
+        if (counts) std::fill(counts, counts + (size_t)n * YK_FILTER_SLOTS, 0u);
+        return YK_OK;
+    }
+    static_assert(YK_FILTER_SLOTS == YK_FILTER_NSLOT && YK_FILTER_RESERVED == YK_FILTER_RES && YK_FAIL_ABSENT == YK_FILTER_ABSENT,
+                  "slot numbers of ykgpu.h and yk_filter.cuh");
+    const int D = e->D;
+    cudaStream_t s = e->stream;
+    const int tiles = (int)((nlive + YK_FILTER_THREADS - 1) / YK_FILTER_THREADS), W = tiles * YK_FILTER_TW;
+    const size_t row_words = (size_t)W + tiles + YK_FILTER_SLOTS + k;
+    const uint32_t chunk = (uint32_t)std::min<size_t>({(size_t)n, FILTER_CHUNK, std::max<size_t>(1, FILTER_WORDS / row_words)});
+    // device buffers are kept between calls and only grow
+    const size_t N = e->maxN;
+    if (e->f_key_in.n < N) {
+        CK(e->f_key_in.alloc(N)); CK(e->f_key_out.alloc(N)); CK(e->f_val_in.alloc(N)); CK(e->f_val_out.alloc(N));
+        size_t tb = 0;
+        CK(cub::DeviceRadixSort::SortPairs(nullptr, tb, e->f_key_in.p, e->f_key_out.p, e->f_val_in.p, e->f_val_out.p, (int)N, 0, 64, s));
+        e->f_cub_bytes = tb;
+        CK(e->f_cub.alloc(tb));
+        CK(e->f_flag.alloc(1)); CK(e->h_f_flag.alloc(1));
+    }
+    CK(grow(e->f_asks, chunk)); CK(grow(e->h_f_asks, chunk));
+    CK(grow(e->f_bits, (size_t)chunk * W)); CK(grow(e->f_tcnt, (size_t)chunk * tiles));
+    CK(grow(e->f_counts, (size_t)chunk * YK_FILTER_SLOTS)); CK(grow(e->h_f_counts, (size_t)chunk * YK_FILTER_SLOTS));
+    if (k) { CK(grow(e->f_out, (size_t)chunk * k)); CK(grow(e->h_f_out, (size_t)chunk * k)); }
+
+    // the cycle's node order at this moment: ascending (score, NodeID rank, index), with the NaN flag
+    CK(cudaMemsetAsync(e->f_flag.p, 0, sizeof(int), s));
+    yk_key_kernel<<<(nlive + 255) / 256, 256, 0, s>>>(D, e->cfg.policy, e->w, e->d_total.p, e->d_avail.p, e->maxN, e->d_by_rank.p,
+                                                      (int)nlive, e->f_key_in.p, e->f_val_in.p, e->f_flag.p);
+    size_t tb = e->f_cub_bytes;
+    CK(cub::DeviceRadixSort::SortPairs(e->f_cub.p, tb, e->f_key_in.p, e->f_key_out.p, e->f_val_in.p, e->f_val_out.p, (int)nlive, 0, 64, s));
+    CK(cudaMemcpyAsync(e->h_f_flag.p, e->f_flag.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+    e->st.other_launches += 11;   // key + cub radix sort, as device_order
+    e->st.d2h_bytes += 4;
+
+    YkFilterArgs a{};
+    a.total = e->d_total.p; a.avail = e->d_avail.p; a.ldn = e->maxN;
+    a.taint = e->d_taint.p; a.label = e->d_label.p; a.flags = e->d_flags.p;
+    a.sorted = e->f_val_out.p; a.nlive = (int)nlive;
+    a.a_req = e->d_areq.p; a.a_tol = e->d_atol.p; a.a_need = e->d_aneed.p; a.a_deny = e->d_adeny.p; a.a_node = e->d_anode.p;
+    a.lda = e->maxA;
+    a.asks = e->f_asks.p; a.allocate = allocate ? 1 : 0;
+    a.bits = e->f_bits.p; a.tilecnt = e->f_tcnt.p; a.counts = e->f_counts.p;
+    a.W = W; a.tiles = tiles;
+    for (uint32_t c0 = 0; c0 < n; c0 += chunk) {
+        const uint32_t rows = std::min(chunk, n - c0);
+        for (uint32_t i = 0; i < rows; ++i) {   // an ask that is not present is sent as YK_NONE: every node counts as YK_FAIL_ABSENT
+            const uint32_t x = asks[c0 + i];
+            e->h_f_asks[i] = e->a_state[x] == yk::ST_ABSENT ? YK_NONE : x;
+        }
+        CK(cudaMemcpyAsync(e->f_asks.p, e->h_f_asks.p, 4 * (size_t)rows, cudaMemcpyHostToDevice, s));
+        CK(cudaMemsetAsync(e->f_counts.p, 0, 4 * (size_t)rows * YK_FILTER_SLOTS, s));
+        // grid.y sized so that tiles x splits fills the device's resident CTA slots about once
+        const int splits = std::max(1, std::min<int>((int)rows, e->slots / tiles));
+        a.rows = (int)rows;
+        a.per = (int)((rows + splits - 1) / splits);
+        launch_filter(D, a, dim3((unsigned)tiles, (unsigned)((rows + a.per - 1) / a.per)), s);
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(e->h_f_counts.p, e->f_counts.p, 4 * (size_t)rows * YK_FILTER_SLOTS, cudaMemcpyDeviceToHost, s));
+        e->st.other_launches += 1;
+        e->st.h2d_bytes += 4 * (size_t)rows;
+        e->st.d2h_bytes += 4 * (size_t)rows * YK_FILTER_SLOTS;
+        if (k) {
+            yk_filter_compact_kernel<<<(rows + 3) / 4, 128, 0, s>>>(e->f_bits.p, e->f_tcnt.p, e->f_counts.p, e->f_val_out.p, (int)rows,
+                                                                    W, tiles, skip, k, e->f_out.p);
+            CK(cudaGetLastError());
+            CK(cudaMemcpyAsync(e->h_f_out.p, e->f_out.p, 4 * (size_t)rows * k, cudaMemcpyDeviceToHost, s));
+            e->st.other_launches += 1;
+            e->st.d2h_bytes += 4 * (size_t)rows * k;
+        }
+        CK(cudaStreamSynchronize(s));
+        if (e->h_f_flag[0]) return e->fail(YK_ERR_RANGE, "yk_filter_nodes: NaN node score (zero total on a weighted resource)");
+        if (k) memcpy(nodes_out + (size_t)c0 * k, e->h_f_out.p, 4 * (size_t)rows * k);
+        if (counts) memcpy(counts + (size_t)c0 * YK_FILTER_SLOTS, e->h_f_counts.p, 4 * (size_t)rows * YK_FILTER_SLOTS);
+        if (n_pass) for (uint32_t i = 0; i < rows; ++i) n_pass[c0 + i] = e->h_f_counts[(size_t)i * YK_FILTER_SLOTS];
+    }
     return YK_OK;
 }
 

@@ -258,7 +258,23 @@ __global__ void yk_p2p_first_kernel(const uint32_t* __restrict__ local, YkPeerFi
 // ---- one (ask,node) answer in the reference's step order, on the device --------------------------------
 // order: core tryNodes (schedulable, FitInNode total) -> tryNode preAllocateCheck (request > 0, available)
 // -> shim Predicates: NodeName, TaintToleration/NodeUnschedulable, NodeAffinity, NodeResourcesFit
-// (predicate_manager.go:339-351 filter order).
+// (predicate_manager.go:339-351 filter order).  The one place that order is written down: yk_evaluate_kernel and
+// yk_filter_kernel (yk_filter.cuh) both call it.  fit_total / fit_avail: request <= max(0, total / available) in every
+// dimension; req_ok: no request below zero and at least one above.  Returns 0 (fits) or YK_FAIL_NODE_NOT_SCHEDULABLE ..
+// YK_FAIL_AFFINITY.
+__host__ __device__ __forceinline__ int yk_first_fail(bool schedulable, bool fit_total, bool req_ok, bool fit_avail,
+                                                      uint32_t want, uint32_t node, uint64_t taint, uint64_t label,
+                                                      uint64_t tol, uint64_t need, uint64_t deny, int allocate) {
+    if (!schedulable) return 1;
+    if (!fit_total) return 2;
+    if (!req_ok) return 3;
+    if (allocate && !fit_avail) return 4;   // reservation phase (Allocate = false): no NodeResourcesFit, no available check
+    if (want != YK_NONE_U32 && want != node) return 5;
+    if (taint & ~tol) return 6;
+    if ((label & need) != need || (label & deny)) return 7;
+    return 0;
+}
+
 __global__ void yk_evaluate_kernel(int D, const int64_t* __restrict__ total, const int64_t* __restrict__ avail,
                                    size_t ldn, const uint64_t* __restrict__ taint, const uint64_t* __restrict__ label,
                                    const uint32_t* __restrict__ flags, const int64_t* __restrict__ a_req,
@@ -266,7 +282,6 @@ __global__ void yk_evaluate_kernel(int D, const int64_t* __restrict__ total, con
                                    const uint64_t* __restrict__ a_deny, const uint32_t* __restrict__ a_node, size_t lda,
                                    uint32_t ask, uint32_t node, int allocate, int* __restrict__ out) {
     if (threadIdx.x || blockIdx.x) return;
-    int r = 0;
     bool pos = false, neg = false, fit_total = true, fit_avail = true;
     for (int k = 0; k < D; ++k) {
         int64_t q = a_req[(size_t)k * lda + ask];
@@ -276,14 +291,8 @@ __global__ void yk_evaluate_kernel(int D, const int64_t* __restrict__ total, con
         if (q > (t < 0 ? 0 : t)) fit_total = false;
         if (q > (a < 0 ? 0 : a)) fit_avail = false;
     }
-    if (!(flags[node] & 1u)) r = 1;
-    else if (!fit_total) r = 2;
-    else if (neg || !pos) r = 3;
-    else if (allocate && !fit_avail) r = 4;   // reservation phase (Allocate = false): no NodeResourcesFit, no available check
-    else if (a_node[ask] != YK_NONE_U32 && a_node[ask] != node) r = 5;
-    else if (taint[node] & ~a_tol[ask]) r = 6;
-    else if ((label[node] & a_need[ask]) != a_need[ask] || (label[node] & a_deny[ask])) r = 7;
-    *out = r;
+    *out = yk_first_fail((flags[node] & 1u) != 0, fit_total, pos && !neg, fit_avail, a_node[ask], node, taint[node],
+                         label[node], a_tol[ask], a_need[ask], a_deny[ask], allocate);
 }
 
 // ---- preemption victim search (predicate_manager.go:137-175), one warp per query ---------------------

@@ -16,11 +16,14 @@ YK_NONE = 0xFFFFFFFF
 ST_PENDING, ST_ALLOCATED, ST_NOFIT, ST_SKIPPED, ST_SLOWPATH, ST_INVALID = range(6)
 ST_ABSENT = 255
 YK_ERR_CUDA = -2
+FILTER_SLOTS = 11          # yk_filter_nodes counts: 0 passes, 1..9 YK_FAIL_*, 10 node reserved
+FILTER_RESERVED = 10
 
 EXPORTS = [
     "yk_abi_version", "yk_create", "yk_destroy", "yk_nodes_upsert", "yk_nodes_remove", "yk_queues_set", "yk_queues_priority",
     "yk_apps_upsert", "yk_apps_remove", "yk_apps_user", "yk_user_limits_set", "yk_asks_upsert", "yk_asks_remove", "yk_release", "yk_cycle",
-    "yk_ask_states", "yk_nodes_available", "yk_evaluate", "yk_evaluate_reserve", "yk_node_scores", "yk_preemption_search", "yk_set_exchange",
+    "yk_ask_states", "yk_nodes_available", "yk_evaluate", "yk_evaluate_reserve", "yk_node_scores", "yk_filter_nodes",
+    "yk_preemption_search", "yk_set_exchange",
     "yk_peer_export", "yk_peer_import", "yk_peer_enable", "yk_stats",
     "yk_stats_reset", "yk_strerror", "yk_last_error",
 ]
@@ -286,6 +289,18 @@ class Engine:
         out = np.zeros(idx.size, dtype=np.float64)
         self._ck(self._lib.yk_node_scores(self._h, C.c_uint32(idx.size), _p(idx), _p(out)))
         return out
+
+    def filter_nodes(self, asks, k=0, skip=0, allocate=True):
+        """-> (nodes[n][k], n_pass[n], counts[n][FILTER_SLOTS]) uint32: per ask, the passing nodes of pass rank skip .. skip+k-1
+        in the cycle's node order (YK_NONE past the end), how many pass, and every present node's first failing step"""
+        asks = _arr(asks, np.uint32)
+        n = asks.size
+        nodes = np.zeros((n, k), dtype=np.uint32)
+        n_pass = np.zeros(n, dtype=np.uint32)
+        counts = np.zeros((n, FILTER_SLOTS), dtype=np.uint32)
+        self._ck(self._lib.yk_filter_nodes(self._h, C.c_uint32(n), _p(asks), C.c_int(1 if allocate else 0), C.c_uint32(skip),
+                                           C.c_uint32(k), _p(nodes) if k else None, _p(n_pass), _p(counts)))
+        return nodes, n_pass, counts
 
     def preemption_search(self, ask, node, victim_req_lists, start):
         """victim_req_lists: per query an [n_victims][D] array of what each victim gives back -> index per query"""

@@ -1,14 +1,13 @@
 // Host emulation of the device-resident ordered commit for the CPU test suite: csrc/yk_lattice.h is single-source -- nvcc
 // turns it into yk_lattice_kernel, g++ turns the SAME code into plain loops -- so the lattice algorithm (bound, element
 // order, acceptance rows, chain, gang snapshots, capacity bound, order patch) is fuzzed against the oracle here without a
-// GPU.  The driver around it is the real ordering engine (csrc/yk_orderer.hpp) and the real meta builder
-// (csrc/yk_lattice_host.hpp).  Test infrastructure: the product only ever runs the kernel.
+// GPU.  The driver around it is the engine's own: the real ordering engine (csrc/yk_orderer.hpp) and the batch loop,
+// segment loop and uniform-run attempts of csrc/yk_lattice_host.hpp.  Test infrastructure: the product only ever runs the
+// kernels.
 //
-// Where the engine hands a batch over to its host commit (status HANDOFF: a gang that cannot be placed from the front of
-// the order), this shim finishes the batch with a plain sequential first-fit over the current order instead.
+// Where the engine hands the rest of the cycle over to its host commit (status HANDOFF: a gang that cannot be placed from
+// the front of the order), this shim runs the same batch loop with a plain sequential first fit over the current order.
 #include "../../yunikorn_k8shim_b200/csrc/yk_lattice_host.hpp"
-#include "../../yunikorn_k8shim_b200/csrc/yk_uniform.h"
-#include "../../yunikorn_k8shim_b200/csrc/yk_orderer.hpp"
 
 #include <algorithm>
 #include <chrono>
@@ -33,76 +32,6 @@ static int g_un_min = 0, g_un_depth = 0;
 extern "C" void host_set_uniform(int min_run, int first_depth) { g_un_min = min_run; g_un_depth = first_depth; }
 
 namespace {
-
-// The uniform-run path as the engine drives it (csrc/yk_engine.cu lt_uniform), with the kernels of yk_uniform.cuh replaced by
-// loops over the same per-item bodies and the two cub radix sorts by std::stable_sort.
-template <int D>
-int uniform_host(const yklt::Args& la, const uint32_t* asks, int off, int R, bool has_gang, uint32_t* res, size_t* consumed, uint64_t* stats) {
-    const int nlive = la.nlive;
-    *consumed = 0;
-    if (nlive == 0 || R == 0) return ykun::U_FALLBACK;
-    const uint32_t ask = asks[off];
-    std::vector<uint32_t> byrank((size_t)nlive);
-    {
-        const yklt::Ent* e = la.ord[*la.cur & 1];
-        std::vector<uint64_t> rn((size_t)nlive);
-        for (int p = 0; p < nlive; ++p) rn[(size_t)p] = e[p].rn;
-        std::sort(rn.begin(), rn.end());
-        for (int p = 0; p < nlive; ++p) byrank[(size_t)p] = (uint32_t)rn[(size_t)p];
-    }
-    uint32_t max_node = 0;
-    for (uint32_t n : byrank) max_node = std::max(max_node, n);
-    std::vector<uint32_t> cnt((size_t)max_node + 1, 0);
-    std::vector<unsigned long long> bk((size_t)nlive), rkey((size_t)nlive), rrn((size_t)nlive), okey((size_t)nlive), orn((size_t)nlive);
-    ykun::Globals g;
-    ykun::Args a{};
-    a.policy = la.policy;
-    for (int k = 0; k < 8; ++k) { a.w[k] = la.w[k]; a.req[k] = k < D ? la.a_req[(size_t)k * la.lda + ask] : 0; }
-    a.rec = la.rec; a.RS = la.RS; a.ord[0] = la.ord[0]; a.ord[1] = la.ord[1]; a.cur = la.cur; a.nlive = nlive; a.byrank = byrank.data();
-    a.tol = la.a_tol[ask]; a.need = la.a_need[ask]; a.deny = la.a_deny[ask]; a.want = la.a_node[ask];
-    a.R = R; a.insensitive = la.insensitive; a.has_gang = has_gang ? 1 : 0;
-    a.bk = bk.data(); a.cnt = cnt.data(); a.rkey = rkey.data(); a.rrn = rrn.data(); a.okey = okey.data(); a.orn = orn.data();
-    a.res = res + off; a.g = &g;
-    int L = g_un_depth > 0 ? g_un_depth : ykun::first_depth(R, nlive);
-    for (;;) {
-        if ((size_t)L * (size_t)nlive > ((size_t)4 << 20)) return ykun::U_FALLBACK;
-        a.L = L;
-        const size_t ne = (size_t)nlive * (size_t)L;
-        std::vector<unsigned long long> ekey(ne), skey(ne);
-        std::vector<uint32_t> enode(ne), snode(ne), idx(ne);
-        a.ekey = ekey.data(); a.enode = enode.data(); a.skey = skey.data(); a.snode = snode.data();
-        g.bkey = ykun::KEY_INF; g.brank = ykun::KEY_INF; g.last_key = 0; g.last_rank = 0; g.valid = 0; g.nan = 0; g.status = ykun::U_RETRY; g.consumed = 0;
-        for (long long x = 0; x < (long long)ne; ++x) {
-            const ykun::DepthOut o = ykun::element_item<D>(a, x);
-            g.valid += o.valid;
-            if (o.bk < g.bkey) g.bkey = o.bk;
-            if (o.nan) g.nan = 1;
-        }
-        for (int i = 0; i < nlive; ++i) { const unsigned long long r = ykun::brank_item<D>(a, i, g.bkey); if (r < g.brank) g.brank = r; }
-        for (size_t x = 0; x < ne; ++x) idx[x] = (uint32_t)x;
-        std::stable_sort(idx.begin(), idx.end(), [&](uint32_t x, uint32_t y) { return ekey[x] < ekey[y]; });
-        for (size_t x = 0; x < ne; ++x) { skey[x] = ekey[idx[x]]; snode[x] = enode[idx[x]]; }
-        for (int q = 0; q < R; ++q) ykun::select_item<D>(a, q, g.valid);
-        ykun::decide(a);
-        int nan_after = 0;
-        for (int i = 0; i < nlive; ++i) { ykun::apply_item<D>(a, i, g.status); nan_after |= ykun::rekey_item<D>(a, i); }
-        {
-            std::vector<uint32_t> ix((size_t)nlive);
-            for (int i = 0; i < nlive; ++i) ix[(size_t)i] = (uint32_t)i;
-            std::stable_sort(ix.begin(), ix.end(), [&](uint32_t x, uint32_t y) { return rkey[x] < rkey[y]; });
-            yklt::Ent* o = la.ord[*la.cur & 1];
-            for (int p = 0; p < nlive; ++p) { o[p].key = rkey[ix[(size_t)p]]; o[p].rn = rrn[ix[(size_t)p]]; }
-        }
-        for (uint32_t c : cnt) if (c) return -99;   // counters must be clean after every attempt
-        stats[8] += 1;
-        if (g.status == ykun::U_RETRY) { stats[9] += 1; L *= 4; continue; }
-        if (g.status == ykun::U_NAN || g.status == ykun::U_FALLBACK) return ykun::U_FALLBACK;
-        if (nan_after) return -5;
-        *consumed = (size_t)g.consumed;
-        stats[10] += (uint64_t)g.consumed;
-        return g.status;
-    }
-}
 
 template <int D>
 int run_d(uint32_t policy, const double* weights,
@@ -134,7 +63,7 @@ int run_d(uint32_t policy, const double* weights,
     std::vector<uint32_t> pending(nA);
     for (uint32_t i = 0; i < nA; ++i) pending[i] = i;
     auto now_ns = [] { return (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
-    uint64_t t_begin = now_ns(), t_fill = 0, t_settle = 0, t_finish = 0;
+    uint64_t t_begin = now_ns();
     o.begin_cycle(pending);
     t_begin = now_ns() - t_begin;
     const bool ins = o.insensitive;
@@ -220,113 +149,121 @@ int run_d(uint32_t policy, const double* weights,
         return yk::CNONE;
     };
 
-    std::vector<uint32_t> asks, meta, shp, sig, result;
-    yk::Orderer::Snap snap;
-    size_t bsz = batch;
-    uint32_t n = 0;
-    uint64_t handoffs = 0, batches = 0;
-    uint64_t ustats[11] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};   // [8] uniform attempts, [9] deeper retries, [10] asks decided by uniform runs
-    while (n < max_bindings) {
-        { const uint64_t t0 = now_ns(); o.fill(bsz, (size_t)max_bindings - n, asks, snap); t_fill += now_ns() - t0; }
-        if (o.oversize_gang) {
-            if (bsz < batch) { bsz = batch; o.fill(bsz, (size_t)max_bindings - n, asks, snap); }
-            if (o.oversize_gang) return -1;
-        }
-        if (asks.empty()) break;
-        ++batches;
-        const size_t B = asks.size();
-        meta.resize(B); shp.resize(B); sig.resize(B);
-        yklt::build_meta(ct, a_shape.data(), a_sigid.data(), asks, meta.data(), shp.data(), sig.data());
+    // a uniform run: the engine's attempt loop (ykun::uniform_run) with the kernels of yk_uniform.cuh replaced by loops over
+    // the same per-item bodies and the two cub radix sorts by std::stable_sort
+    std::vector<uint32_t> asks, result, meta(std::max<uint32_t>(nA, 1)), shp(meta.size()), sig(meta.size());
+    yk_stats_t st{};
+    uint64_t attempts = 0;
+    std::vector<uint32_t> byrank(nN);   // the nodes by ascending (NodeID rank, index)
+    for (uint32_t i = 0; i < nN; ++i) byrank[i] = i;
+    std::sort(byrank.begin(), byrank.end(), [&](uint32_t x, uint32_t y) { return n_rank[x] != n_rank[y] ? n_rank[x] < n_rank[y] : x < y; });
+    auto uniform = [&](size_t off, size_t R, bool has_gang, int* ust, size_t* consumed) -> int {
+        const int nlive = (int)nN;
+        std::vector<uint32_t> cnt((size_t)nN, 0);
+        std::vector<unsigned long long> bk((size_t)nlive), rkey((size_t)nlive), rrn((size_t)nlive), okey((size_t)nlive), orn((size_t)nlive);
+        const uint32_t ask = asks[off];
+        ykun::Args a{};
+        a.policy = la.policy;
+        for (int k = 0; k < 8; ++k) { a.w[k] = la.w[k]; a.req[k] = k < D ? la.a_req[(size_t)k * la.lda + ask] : 0; }
+        a.rec = la.rec; a.RS = la.RS; a.ord[0] = la.ord[0]; a.ord[1] = la.ord[1]; a.cur = la.cur; a.nlive = nlive; a.byrank = byrank.data();
+        a.tol = la.a_tol[ask]; a.need = la.a_need[ask]; a.deny = la.a_deny[ask]; a.want = la.a_node[ask];
+        a.R = (int)R; a.insensitive = la.insensitive; a.has_gang = has_gang ? 1 : 0;
+        a.bk = bk.data(); a.cnt = cnt.data(); a.rkey = rkey.data(); a.rrn = rrn.data(); a.okey = okey.data(); a.orn = orn.data();
+        a.res = result.data() + off;
+        auto attempt = [&](int L, ykun::Globals& g) -> int {
+            a.L = L; a.g = &g;
+            const size_t ne = (size_t)nlive * (size_t)L;
+            std::vector<unsigned long long> ekey(ne), skey(ne);
+            std::vector<uint32_t> enode(ne), snode(ne), idx(ne);
+            a.ekey = ekey.data(); a.enode = enode.data(); a.skey = skey.data(); a.snode = snode.data();
+            g.bkey = ykun::KEY_INF; g.brank = ykun::KEY_INF; g.last_key = 0; g.last_rank = 0; g.valid = 0; g.nan = 0; g.status = ykun::U_RETRY; g.consumed = 0;
+            for (long long x = 0; x < (long long)ne; ++x) {
+                const ykun::DepthOut o = ykun::element_item<D>(a, x);
+                g.valid += o.valid;
+                if (o.bk < g.bkey) g.bkey = o.bk;
+                if (o.nan) g.nan = 1;
+            }
+            for (int i = 0; i < nlive; ++i) { const unsigned long long r = ykun::brank_item<D>(a, i, g.bkey); if (r < g.brank) g.brank = r; }
+            for (size_t x = 0; x < ne; ++x) idx[x] = (uint32_t)x;
+            std::stable_sort(idx.begin(), idx.end(), [&](uint32_t x, uint32_t y) { return ekey[x] < ekey[y]; });
+            for (size_t x = 0; x < ne; ++x) { skey[x] = ekey[idx[x]]; snode[x] = enode[idx[x]]; }
+            for (int q = 0; q < (int)R; ++q) ykun::select_item<D>(a, q, g.valid);
+            ykun::decide(a);
+            for (int i = 0; i < nlive; ++i) { ykun::apply_item<D>(a, i, g.status); if (ykun::rekey_item<D>(a, i)) g.nan = 2; }
+            {
+                std::vector<uint32_t> ix((size_t)nlive);
+                for (int i = 0; i < nlive; ++i) ix[(size_t)i] = (uint32_t)i;
+                std::stable_sort(ix.begin(), ix.end(), [&](uint32_t x, uint32_t y) { return rkey[x] < rkey[y]; });
+                yklt::Ent* o = la.ord[*la.cur & 1];
+                for (int p = 0; p < nlive; ++p) { o[p].key = rkey[ix[(size_t)p]]; o[p].rn = rrn[ix[(size_t)p]]; }
+            }
+            for (uint32_t c : cnt) if (c) return -99;   // counters must be clean after every attempt
+            ++attempts;
+            return 0;
+        };
+        const int rc = ykun::uniform_run(D, la.w, a.req, n_total, nN, byrank.data(), nlive, (int)R, g_un_depth, st, attempt, ust, consumed);
+        if (rc) return rc;
+        return *ust == ykun::U_NAN || order_ok() ? 0 : -9;
+    };
+    auto window = [&](size_t off, size_t len, int* status, size_t* consumed) -> int {
+        la.asks = asks.data() + off; la.meta = meta.data() + off; la.shp = shp.data() + off; la.sig = sig.data() + off;
+        la.B = (int)len; la.res = result.data() + off;
+        yklt::lattice_batch<D>(la, *sh);
+        *status = hdr[yklt::H_STATUS];
+        *consumed = (size_t)hdr[yklt::H_CONSUMED];
+        return *status == yklt::ST_NAN || order_ok() ? 0 : -9;
+    };
+    std::vector<ykun::Segment> segs;
+    auto lattice = [&](size_t B, int* status, size_t* consumed) -> int {
         result.assign(B, yk::CNONE);
-        la.asks = asks.data(); la.meta = meta.data(); la.shp = shp.data(); la.sig = sig.data(); la.B = (int)B; la.res = result.data();
-        size_t consumed = 0;
-        if (nN == 0) {
-            consumed = ins ? B : 1;
-            if (!ins && a_gang[asks[0]] != yk::CNONE)
-                while (consumed < B && a_gang[asks[consumed]] == a_gang[asks[0]] && a_app[asks[consumed]] == a_app[asks[0]]) ++consumed;
-        } else {
-            // the engine's lt_batch: uniform runs through the uniform-run path, the stretches between them through the kernel
-            std::vector<ykun::Segment> segs;
-            ykun::plan_segments(meta.data(), shp.data(), sig.data(), (int)B, g_un_min > 0 ? g_un_min : (int)B + 1, segs);
-            int status = yklt::ST_DONE;
-            for (const ykun::Segment& sg : segs) {
-                size_t cons = 0;
-                int st = yklt::ST_DONE;
-                bool windowed = !sg.uniform;
-                if (sg.uniform) {
-                    bool has_gang = false;
-                    for (int i = 0; i < sg.len; ++i) has_gang = has_gang || (meta[(size_t)sg.off + i] & yklt::M_GANG);
-                    const int ust = uniform_host<D>(la, asks.data(), sg.off, sg.len, has_gang, result.data(), &cons, ustats);
-                    if (ust < 0) return ust;
-                    if (ust == ykun::U_FALLBACK) windowed = true;
-                    else st = ust == ykun::U_STOPPED ? yklt::ST_STOPPED : yklt::ST_DONE;
-                }
-                if (windowed) {
-                    la.asks = asks.data() + sg.off; la.meta = meta.data() + sg.off; la.shp = shp.data() + sg.off; la.sig = sig.data() + sg.off;
-                    la.B = sg.len; la.res = result.data() + sg.off;
-                    yklt::lattice_batch<D>(la, *sh);
-                    st = hdr[yklt::H_STATUS];
-                    cons = (size_t)hdr[yklt::H_CONSUMED];
-                }
-                if (st == yklt::ST_NAN) return -5;
-                if (!order_ok()) return -9;
-                consumed = (size_t)sg.off + cons;
-                status = st;
-                if (st != yklt::ST_DONE || cons < (size_t)sg.len) break;
+        return yklt::run_segments(segs, meta.data(), uniform, window, status, consumed);
+    };
+    // after a hand-off: a plain sequential first fit with gang roll-back, the stand-in for the engine's host commit
+    auto sequential = [&](size_t B, int* status, size_t* consumed) -> int {
+        result.assign(B, yk::CNONE);
+        size_t i = 0;
+        bool stop = false;
+        while (i < B && !stop) {   // an ask or a whole gang at a time: all of it placed, or none
+            size_t g1 = i + 1;
+            while (g1 < B && yk::same_gang(o.t, asks[i], asks[g1])) ++g1;
+            const std::vector<int64_t> keep(rec);
+            size_t x = i;
+            while (x < g1 && (result[x] = seq_place(asks[x])) != yk::CNONE) ++x;
+            if (x < g1) {
+                std::copy(keep.begin(), keep.end(), rec.begin());
+                resort();
+                std::fill(result.begin() + i, result.begin() + g1, yk::CNONE);
+                stop = !ins;
             }
-            hdr[yklt::H_STATUS] = status;
-            hdr[yklt::H_CONSUMED] = (int)consumed;
-            if (hdr[yklt::H_STATUS] == yklt::ST_HANDOFF) {
-                ++handoffs;
-                bool stop = false;
-                size_t i = consumed;
-                while (i < B && !stop) {
-                    const uint32_t a = asks[i];
-                    if (a_gang[a] == yk::CNONE) {
-                        result[i] = seq_place(a);
-                        if (result[i] == yk::CNONE && !ins) stop = true;
-                        ++i;
-                        continue;
-                    }
-                    size_t g1 = i;
-                    while (g1 < B && a_gang[asks[g1]] == a_gang[a] && a_app[asks[g1]] == a_app[a]) ++g1;
-                    std::vector<int64_t> keep(rec);
-                    bool okg = true;
-                    for (size_t x = i; x < g1 && okg; ++x) { result[x] = seq_place(asks[x]); okg = result[x] != yk::CNONE; }
-                    if (!okg) {
-                        rec = keep; la.rec = rec.data();
-                        resort();
-                        for (size_t x = i; x < g1; ++x) result[x] = yk::CNONE;
-                        if (!ins) stop = true;
-                    }
-                    i = g1;
-                }
-                consumed = i;
-                for (int k = 0; k < 8; ++k) ub[k] = INT64_MAX;   // a roll-back may have handed capacity back
-            }
+            i = g1;
         }
-        bool failed = false;
-        if (!ins && consumed > 0 && result[consumed - 1] == yk::CNONE) {
-            size_t j = consumed - 1;
-            while (j > 0 && a_gang[asks[j]] != yk::CNONE && a_gang[asks[j - 1]] == a_gang[asks[j]] &&
-                   a_app[asks[j - 1]] == a_app[asks[j]] && result[j - 1] == yk::CNONE) --j;
-            o.rewind(snap, nullptr, asks, j);
-            failed = true;
-        } else if (!ins && consumed < B) {
-            return -12;   // a placement-sensitive batch may only end early on a failure
-        }
-        const uint64_t t_s0 = now_ns();
-        for (size_t i = 0; i < consumed; ++i) {
-            const uint32_t a = asks[i];
-            if (result[i] == yk::CNONE) { if (ins) o.fail_in_place(a); continue; }
-            o.confirm(a);
-            out_ask[n] = a; out_node[n] = result[i]; ++n;
-        }
-        t_settle += now_ns() - t_s0;
-        if (ins && consumed < B) return -13;
-        bsz = failed ? std::max<size_t>(std::min<size_t>(64, batch), bsz / 4) : std::min<size_t>(batch, bsz * 2);
+        *status = stop ? yklt::ST_STOPPED : yklt::ST_DONE;
+        *consumed = i;
+        return 0;
+    };
+    uint32_t n = 0;
+    auto bind = [&](uint32_t a, uint32_t node) { out_ask[n] = a; out_node[n] = node; ++n; };
+    // YK_ERR_RANGE = -5: a NaN score; YK_ERR_ARG = -1: a gang no batch holds; a batch that ended early without a failure
+    // is -13 in an insensitive order, -12 in a placement-sensitive one
+    auto fail = [&](int code, const char*) { return code == YK_ERR_CUDA ? (ins ? -13 : -12) : code; };
+
+    const uint64_t t_loop = now_ns();
+    yk::Orderer::Snap snap;
+    bool plan_ready = false, handoff = false;
+    yklt::Loop lp{o, ct, a_shape.data(), a_sigid.data(), asks, snap, result, meta.data(), shp.data(), sig.data(), segs, plan_ready,
+                  g_un_min, nN == 0, batch, max_bindings, n, st};
+    size_t bsz = batch;
+    if (!yk::fill_batch(o, bsz, batch, max_bindings, asks, snap, st)) return -1;
+    int rc = yklt::device_commit(lp, lattice, bind, fail, handoff);
+    if (!rc && handoff) {   // the engine's path: the rest of the cycle on the host commit, never back on the device
+        lp.min_run = 0;
+        bsz = batch;
+        if (!yk::fill_batch(o, bsz, batch, (size_t)max_bindings - n, asks, snap, st)) return -1;
+        rc = yklt::device_commit(lp, sequential, bind, fail, handoff);
     }
-    t_finish = now_ns();
+    if (rc) return rc;
+    const uint64_t t_batches = now_ns() - t_loop;
+    uint64_t t_finish = now_ns();
     o.finish();
     t_finish = now_ns() - t_finish;
     *n_out = n;
@@ -336,9 +273,10 @@ int run_d(uint32_t policy, const double* weights,
     if (stats_out) {
         stats_out[0] = (uint64_t)hdr[yklt::H_SUBRUNS]; stats_out[1] = (uint64_t)hdr[yklt::H_FULLSCANS]; stats_out[2] = (uint64_t)hdr[yklt::H_SORTS];
         stats_out[3] = (uint64_t)hdr[yklt::H_ELEMS]; stats_out[4] = (uint64_t)hdr[yklt::H_QUICK]; stats_out[5] = (uint64_t)hdr[yklt::H_ESC];
-        stats_out[6] = handoffs; stats_out[7] = batches;
-        stats_out[8] = ustats[8]; stats_out[9] = ustats[9]; stats_out[10] = ustats[10];
-        stats_out[11] = t_begin; stats_out[12] = t_fill; stats_out[13] = t_settle; stats_out[14] = t_finish;   // ns (development aid)
+        stats_out[6] = st.lattice_handoffs; stats_out[7] = st.batches;
+        stats_out[8] = attempts; stats_out[9] = st.uniform_retries; stats_out[10] = st.uniform_asks;
+        // ns (development aid): orderer setup, orderer fill + rewind, the batch loops, finish
+        stats_out[11] = t_begin; stats_out[12] = (uint64_t)(st.host_ms[2] * 1e6); stats_out[13] = t_batches; stats_out[14] = t_finish;
     }
     return 0;
 }

@@ -78,13 +78,17 @@ def test_binpacking_is_left_to_the_host_commit(lshim):
 
 def test_full_cluster_and_gang_rollbacks(lshim, oracle):
     """over-committed clusters: certain NOFITs by full scan, the capacity bound that rejects later asks without one, gangs
-    that do not fit (decided on the device when no node takes the first member, handed over otherwise)"""
+    that do not fit (decided on the device when no node takes the first member, handed over otherwise); with a max on the
+    queue the order is placement-sensitive, so a failed gang ends its batch and the orderer rewinds to its first member"""
     for seed in range(6):
         for fill in (1.05, 2.0):
-            st = []
-            s = synth.gangs(120, 40, 5, seed=seed, fill=fill)
-            want = check(lshim, oracle, s, tag=(seed, fill), batch=1000, stats=st)
-            assert want is not None and (want["state"] == 2).sum() > 0
+            for quota in (False, True):
+                st = []
+                s = synth.gangs(120, 40, 5, seed=seed, fill=fill)
+                if quota:
+                    s.q_max[-1, 0] = 1 << 60   # never binds
+                want = check(lshim, oracle, s, tag=(seed, fill, quota), batch=1000, stats=st)
+                assert want is not None and (want["state"] == 2).sum() > 0
     # a gang whose members differ in what they request never reaches the lattice commit
     assert run(lshim, synth.poisoned_gangs(3))[0] == INELIGIBLE
 
@@ -163,13 +167,25 @@ def test_uniform_reference_shape(lshim, oracle):
     """the reference's benchmark shape, small: identical nodes, identical pods -> every key ties across nodes at every depth"""
     for nodes, apps, tasks in ((50, 4, 125), (7, 3, 50), (100, 10, 110)):
         s = synth.reference_shape(nodes, apps, tasks)
-        for uniform in ((16, 0), (16, 1), (16, 3)):
+        for uniform in ((16, 0), (16, 1), (16, 3), (16, 1 << 20)):   # a first depth past every node's capacity is cut back to it
             st = []
             want = check(lshim, oracle, s, tag=(nodes, uniform), batch=1 << 20, stats=st, uniform=uniform)
             assert want is not None
             assert st[0]["uniform_asks"] == len(want["ask"]) == s.n_asks and st[0]["subruns"] == 0
             if uniform[1] == 1:
                 assert st[0]["uniform_retries"] > 0
+
+
+@pytest.mark.parametrize("nodes,apps,tasks", [(20, 4, 100), (50, 2, 100)])
+def test_uniform_flat_request_takes_one_attempt(lshim, oracle, nodes, apps, tasks):
+    """{pods: 1} requests no weighted resource, so no key moves and the run fills the front nodes to the brim: the first
+    attempt generates a node's whole capacity (110 here, more than the mean-share depth) and never retries"""
+    s = synth.kwok(nodes, apps, tasks, variant="bare")
+    st = []
+    want = check(lshim, oracle, s, batch=1 << 20, stats=st, uniform=(16, 0))
+    assert want is not None and len(want["ask"]) == s.n_asks
+    assert st[0]["uniform_asks"] == s.n_asks and st[0]["subruns"] == 0
+    assert st[0]["uniform_attempts"] == 1 and st[0]["uniform_retries"] == 0
 
 
 def test_uniform_run_overflows_the_cluster(lshim, oracle):

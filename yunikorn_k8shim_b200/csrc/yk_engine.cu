@@ -476,20 +476,18 @@ int initial_order(yk_engine* e) {
 }
 
 // ---- uniform runs on the device (yk_uniform.h / yk_uniform.cuh) -------------------------------------------------------
-constexpr size_t UN_EMAX = (size_t)4 << 20;   // generated elements per attempt at most (nodes x depth)
-
 int un_ensure(yk_engine* e) {
     if (e->un_alloc) return YK_OK;
     const size_t N = e->maxN;
     for (int b = 0; b < 2; ++b) {
-        CK(e->d_un_ekey[b].alloc(UN_EMAX)); CK(e->d_un_enode[b].alloc(UN_EMAX));
+        CK(e->d_un_ekey[b].alloc(ykun::UN_EMAX)); CK(e->d_un_enode[b].alloc(ykun::UN_EMAX));
         CK(e->d_un_rkey[b].alloc(N)); CK(e->d_un_rrn[b].alloc(N));
     }
     CK(e->d_un_bk.alloc(N)); CK(e->d_un_cnt.alloc(N));
     CK(e->d_un_g.alloc(1)); CK(e->h_un_g.alloc(1));
     CK(cudaMemsetAsync(e->d_un_cnt.p, 0, sizeof(uint32_t) * std::max<size_t>(N, 1), e->stream));
     size_t t0 = 0, t1 = 0;
-    CK(cub::DeviceRadixSort::SortPairs(nullptr, t0, e->d_un_ekey[0].p, e->d_un_ekey[1].p, e->d_un_enode[0].p, e->d_un_enode[1].p, (int)UN_EMAX, 0, 64, e->stream));
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, t0, e->d_un_ekey[0].p, e->d_un_ekey[1].p, e->d_un_enode[0].p, e->d_un_enode[1].p, (int)ykun::UN_EMAX, 0, 64, e->stream));
     CK(cub::DeviceRadixSort::SortPairs(nullptr, t1, e->d_un_rkey[0].p, e->d_un_rkey[1].p, e->d_un_rrn[0].p, e->d_un_rrn[1].p, (int)std::max<size_t>(N, 1), 0, 64, e->stream));
     e->un_cub_bytes = std::max(t0, t1);
     CK(e->d_un_cub.alloc(e->un_cub_bytes));
@@ -539,13 +537,10 @@ int un_reorder(yk_engine* e) {
     return YK_OK;
 }
 
-// One uniform run: entries [off, off + R) of the staged batch (h_lt_asks; results land in d_lt_res at the same offset).
-// status = ykun::U_DONE / U_STOPPED with *consumed entries decided, or U_FALLBACK: nothing was applied, the windowed kernel
-// takes the run.
-int lt_uniform(yk_engine* e, size_t off, size_t R, bool insensitive, bool has_gang, int* status, size_t* consumed) {
-    *status = ykun::U_FALLBACK; *consumed = 0;
+// One uniform run: entries [off, off + R) of the staged batch (h_lt_asks; results land in d_lt_res at the same offset),
+// through ykun::uniform_run with un_attempt as the attempt.
+int lt_uniform(yk_engine* e, size_t off, size_t R, bool has_gang, int* status, size_t* consumed) {
     const int nlive = (int)e->nlive;
-    if (nlive == 0 || R == 0) return YK_OK;
     int rc = un_ensure(e);
     if (rc) return rc;
     cudaStream_t s = e->stream;
@@ -556,32 +551,12 @@ int lt_uniform(yk_engine* e, size_t off, size_t R, bool insensitive, bool has_ga
     a.rec = e->d_rec.p; a.RS = e->lt_RS; a.ord[0] = e->d_ord[0].p; a.ord[1] = e->d_ord[1].p; a.cur = e->d_lt_cur.p;
     a.nlive = nlive; a.byrank = e->d_by_rank.p;   // live nodes by ascending (NodeID rank, index): upload_tables
     a.tol = e->a_tol[ask]; a.need = e->a_need[ask]; a.deny = e->a_deny[ask]; a.want = e->a_node[ask];
-    a.R = (int)R; a.insensitive = insensitive ? 1 : 0; a.has_gang = has_gang ? 1 : 0;
+    a.R = (int)R; a.insensitive = e->ord.insensitive ? 1 : 0; a.has_gang = has_gang ? 1 : 0;
     a.ekey = e->d_un_ekey[0].p; a.skey = e->d_un_ekey[1].p; a.enode = e->d_un_enode[0].p; a.snode = e->d_un_enode[1].p;
     a.bk = e->d_un_bk.p; a.cnt = e->d_un_cnt.p;
     a.rkey = e->d_un_rkey[0].p; a.okey = e->d_un_rkey[1].p; a.rrn = e->d_un_rrn[0].p; a.orn = e->d_un_rrn[1].p;
     a.res = e->d_lt_res.p + off; a.g = e->d_un_g.p;
-    int L = ykun::first_depth((int)R, nlive);
-    // no node takes the request more often than its TOTAL allows: beyond that depth nothing is ever cut
-    int64_t capmax = 0;
-    for (uint32_t i = 0; i < e->nlive; ++i) {
-        const uint32_t n = e->by_rank[i];
-        int64_t tot[8];
-        for (int k = 0; k < e->D; ++k) tot[k] = e->n_total[(size_t)k * e->maxN + n];
-        capmax = std::max(capmax, ykun::cap_of_d(e->D, true, tot, tot, a.req, (int64_t)R));
-    }
-    int Lmax = 1;
-    while ((int64_t)Lmax < capmax) Lmax <<= 1;
-    {   // a request with no weighted dimension leaves every key where it is: the run fills the first nodes (by key, NodeID) to
-        // the brim, so the depth that matters is a node's whole capacity, not the mean share
-        bool flat = true;
-        for (int k = 0; k < e->D; ++k) if (e->w.w[k] != 0.0 && a.req[k] != 0) flat = false;
-        if (flat) L = Lmax;
-    }
-    if (e->un_depth > 0) L = e->un_depth;   // testing knob: a shallow first attempt makes the retry path reachable
-    L = std::min(L, Lmax);
-    for (;;) {
-        if ((size_t)L * (size_t)nlive > UN_EMAX) return YK_OK;   // too deep for the element buffers: fallback
+    auto attempt = [&](int L, ykun::Globals& g) -> int {
         a.L = L;
         CK(cudaEventRecord(e->ev_l0, s));
         CK(un_attempt(e, a));
@@ -594,19 +569,13 @@ int lt_uniform(yk_engine* e, size_t off, size_t R, bool insensitive, bool has_ga
         e->st.lattice_launches += 1;
         e->st.other_launches += 16;   // 6 kernels of yk_uniform.cuh + one cub radix sort (histogram, exclusive sum, 8 onesweep passes)
         e->st.d2h_bytes += sizeof(ykun::Globals);
-        const ykun::Globals& g = e->h_un_g[0];
-        if (g.status == ykun::U_RETRY) {   // deeper; past Lmax only if a node's available exceeds its total (the buffers end it)
-            e->st.uniform_retries++;
-            L = L < Lmax ? (int)std::min<int64_t>((int64_t)L * 4, (int64_t)Lmax) : L * 4;
-            continue;
-        }
-        if (g.status == ykun::U_NAN || g.status == ykun::U_FALLBACK) return YK_OK;
-        if (g.nan) return e->fail(YK_ERR_RANGE, "NaN node score after commit");
-        *status = g.status; *consumed = (size_t)g.consumed;
-        e->un_ord_stale = true;
-        e->st.uniform_runs++; e->st.uniform_asks += (uint64_t)g.consumed; e->st.uniform_elements += (uint64_t)L * (uint64_t)nlive;
+        g = e->h_un_g[0];
         return YK_OK;
-    }
+    };
+    rc = ykun::uniform_run(e->D, e->w.w, a.req, e->n_total.p, e->maxN, e->by_rank.p, nlive, (int)R, e->un_depth, e->st, attempt,
+                           status, consumed);
+    if (*status == ykun::U_DONE || *status == ykun::U_STOPPED) e->un_ord_stale = true;
+    return rc;
 }
 
 // ---- device-resident ordered commit (yk_lattice.h) -------------------------------------------------------------------
@@ -629,10 +598,8 @@ int lt_prepare(yk_engine* e) {
     return YK_OK;
 }
 
-// One batch through the device commit: asks + their three words up (already in the pinned staging buffers), node indices +
-// header back.  Uniform runs of at least un_min entries go through lt_uniform, the stretches between them through
-// yk_lattice_kernel; h_lt_hdr[H_STATUS / H_CONSUMED] describe the whole batch afterwards.  Blocks until it is decided.
-int lt_window(yk_engine* e, size_t off, size_t B, bool insensitive) {
+// One stretch [off, off + B) of the staged batch through yk_lattice_kernel; its header comes back into h_lt_hdr.
+int lt_window(yk_engine* e, size_t off, size_t B) {
     cudaStream_t s = e->stream;
     { const int rco = un_reorder(e); if (rco) return rco; }
     yklt::Args a{};
@@ -642,7 +609,7 @@ int lt_window(yk_engine* e, size_t off, size_t B, bool insensitive) {
     a.nlive = (int)e->nlive;
     a.a_req = e->d_areq.p; a.lda = e->maxA; a.a_tol = e->d_atol.p; a.a_need = e->d_aneed.p; a.a_deny = e->d_adeny.p; a.a_node = e->d_anode.p;
     a.asks = e->d_lt_asks.p + off; a.meta = e->d_lt_meta.p + off; a.shp = e->d_lt_shp.p + off; a.sig = e->d_lt_sig.p + off; a.B = (int)B;
-    a.res = e->d_lt_res.p + off; a.hdr = e->d_lt_hdr.p; a.ub = e->d_lt_ub.p; a.insensitive = insensitive ? 1 : 0;
+    a.res = e->d_lt_res.p + off; a.hdr = e->d_lt_hdr.p; a.ub = e->d_lt_ub.p; a.insensitive = e->ord.insensitive ? 1 : 0;
     a.prof = e->lt_prof ? e->d_lt_prof.p : nullptr;
     CK(cudaEventRecord(e->ev_l0, s));
     launch_lattice(e->D, a, e->lt_smem, s);
@@ -658,55 +625,37 @@ int lt_window(yk_engine* e, size_t off, size_t B, bool insensitive) {
     return YK_OK;
 }
 
-int lt_batch(yk_engine* e, size_t B, bool insensitive) {
+// One batch of slot[0] (segments planned in e->un_segs) through yklt::run_segments; the decided entries' nodes land in
+// `result`.  Blocks until it is decided.
+int lt_batch(yk_engine* e, size_t B, int* status, size_t* done, std::vector<uint32_t>& result) {
     cudaStream_t s = e->stream;
-    // the segments (e->un_segs) were planned by the caller; only the windowed kernel reads the per-entry words
-    bool staged = false;
-    auto stage = [&]() -> int {
-        if (staged) return YK_OK;
-        CK(cudaMemcpyAsync(e->d_lt_asks.p, e->h_lt_asks.p, 4 * B, cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(e->d_lt_meta.p, e->h_lt_meta.p, 4 * B, cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(e->d_lt_shp.p, e->h_lt_shp.p, 4 * B, cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(e->d_lt_sig.p, e->h_lt_sig.p, 4 * B, cudaMemcpyHostToDevice, s));
-        e->st.h2d_bytes += 16 * B;
-        staged = true;
+    memcpy(e->h_lt_asks.p, e->slot[0].asks.data(), 4 * B);
+    bool staged = false;   // only the windowed kernel reads the per-entry words
+    auto uniform = [&](size_t off, size_t len, bool has_gang, int* ust, size_t* consumed) { return lt_uniform(e, off, len, has_gang, ust, consumed); };
+    auto window = [&](size_t off, size_t len, int* st, size_t* consumed) -> int {
+        if (!staged) {
+            CK(cudaMemcpyAsync(e->d_lt_asks.p, e->h_lt_asks.p, 4 * B, cudaMemcpyHostToDevice, s));
+            CK(cudaMemcpyAsync(e->d_lt_meta.p, e->h_lt_meta.p, 4 * B, cudaMemcpyHostToDevice, s));
+            CK(cudaMemcpyAsync(e->d_lt_shp.p, e->h_lt_shp.p, 4 * B, cudaMemcpyHostToDevice, s));
+            CK(cudaMemcpyAsync(e->d_lt_sig.p, e->h_lt_sig.p, 4 * B, cudaMemcpyHostToDevice, s));
+            e->st.h2d_bytes += 16 * B;
+            staged = true;
+        }
+        const int rc = lt_window(e, off, len);
+        if (rc) return rc;
+        *st = e->h_lt_hdr[yklt::H_STATUS];
+        *consumed = (size_t)e->h_lt_hdr[yklt::H_CONSUMED];
+        if (*consumed > len) return e->fail(YK_ERR_CUDA, "lattice kernel returned a bad header");
         return YK_OK;
     };
-    int status = yklt::ST_DONE;
-    size_t done = 0;
-    for (const ykun::Segment& sg : e->un_segs) {
-        size_t consumed = 0;
-        int st = yklt::ST_DONE;
-        bool windowed = !sg.uniform;
-        if (sg.uniform) {
-            bool has_gang = false;
-            for (int i = 0; i < sg.len && !has_gang; ++i) has_gang = (e->h_lt_meta[(size_t)sg.off + i] & yklt::M_GANG) != 0;
-            int ust = ykun::U_FALLBACK;
-            const int rc = lt_uniform(e, (size_t)sg.off, (size_t)sg.len, insensitive, has_gang, &ust, &consumed);
-            if (rc) return rc;
-            if (ust == ykun::U_FALLBACK) windowed = true;
-            else st = ust == ykun::U_STOPPED ? yklt::ST_STOPPED : yklt::ST_DONE;
-        }
-        if (windowed) {
-            const int rcs = stage();
-            if (rcs) return rcs;
-            const int rc = lt_window(e, (size_t)sg.off, (size_t)sg.len, insensitive);
-            if (rc) return rc;
-            st = e->h_lt_hdr[yklt::H_STATUS];
-            consumed = (size_t)e->h_lt_hdr[yklt::H_CONSUMED];
-            if (consumed > (size_t)sg.len) return e->fail(YK_ERR_CUDA, "lattice kernel returned a bad header");
-        }
-        done = (size_t)sg.off + consumed;
-        status = st;
-        if (st != yklt::ST_DONE || consumed < (size_t)sg.len) break;
-    }
-    e->h_lt_hdr[yklt::H_STATUS] = status;
-    e->h_lt_hdr[yklt::H_CONSUMED] = (int)done;
-    if (done) {
-        CK(cudaMemcpyAsync(e->h_lt_res.p, e->d_lt_res.p, 4 * done, cudaMemcpyDeviceToHost, s));
+    const int rc = yklt::run_segments(e->un_segs, e->h_lt_meta.p, uniform, window, status, done);
+    if (rc) return rc;
+    if (*done) {
+        CK(cudaMemcpyAsync(e->h_lt_res.p, e->d_lt_res.p, 4 * *done, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
-        e->st.d2h_bytes += 4 * done;
+        e->st.d2h_bytes += 4 * *done;
     }
+    result.assign(e->h_lt_res.p, e->h_lt_res.p + B);
     return YK_OK;
 }
 
@@ -1481,115 +1430,39 @@ struct Cycle {
     std::vector<uint32_t> result;
 };
 
-// Decided entries [0, consumed) of a batch: orderer bookkeeping + bindings out.  `failed` = the batch ended on an ask /
-// gang that found no node in a placement-sensitive order (the orderer is rewound to just before it).
-void settle(yk_engine* e, Cycle& c, Slot& A, Slot* later, bool later_forked, size_t consumed, bool ins, bool& failed) {
-    failed = false;
-    const std::vector<uint32_t>& result = c.result;
-    if (!ins && consumed > 0 && result[consumed - 1] == YK_NONE) {
-        const double t_r = now_ms();
-        size_t j = consumed - 1;   // first entry of the failed ask / gang
-        while (j > 0 && e->a_gang[A.asks[j]] != YK_NONE && e->a_gang[A.asks[j - 1]] == e->a_gang[A.asks[j]] &&
-               e->a_app[A.asks[j - 1]] == e->a_app[A.asks[j]] && result[j - 1] == YK_NONE) --j;
-        // the speculated fill is undone even when it produced no batch: it may still have marked asks (headroom skips)
-        e->ord.rewind(A.snap, later_forked && later ? &later->snap : nullptr, A.asks, j);
-        e->st.host_ms[2] += now_ms() - t_r;
-        failed = true;
-    }
-    for (size_t i = 0; i < consumed; ++i) {
-        const uint32_t a = A.asks[i];
-        if (result[i] == YK_NONE) {
-            if (ins) e->ord.fail_in_place(a);
-            e->st.nofit++;
-            continue;
-        }
-        e->ord.confirm(a);
-        e->a_bound[a] = result[i];
-        c.out[c.n].ask = a; c.out[c.n].node = result[i];
-        ++c.n;
-        e->st.allocations++;
-    }
+// one binding: out to the caller, and remembered for yk_release
+void bind_one(yk_engine* e, Cycle& c, uint32_t a, uint32_t node) {
+    e->a_bound[a] = node;
+    c.out[c.n].ask = a; c.out[c.n].node = node;
+    ++c.n;
 }
 
 // fill one batch; YK_ERR_ARG when a gang cannot fit any batch
 int fill_batch(yk_engine* e, size_t& bsz, size_t bmax, size_t cap_user, Slot& sl, yk_stats_t& st) {
-    sl.asks.clear(); sl.B = 0; sl.nchunks = 0;
-    if (cap_user == 0) return YK_OK;
-    const double t_f = now_ms();
-    e->ord.fill(bsz, cap_user, sl.asks, sl.snap);
-    st.host_ms[2] += now_ms() - t_f;
-    if (e->ord.oversize_gang) {
-        if (bsz < bmax) { bsz = bmax; e->ord.fill(bsz, cap_user, sl.asks, sl.snap); }
-        if (e->ord.oversize_gang)
-            return e->fail(YK_ERR_ARG, "yk_cycle: a gang has more members than the sweep batch (raise yk_config.batch)");
-    }
+    sl.B = 0; sl.nchunks = 0;
+    if (!yk::fill_batch(e->ord, bsz, bmax, cap_user, sl.asks, sl.snap, st))
+        return e->fail(YK_ERR_ARG, yk::GANG_TOO_BIG);
     return YK_OK;
 }
 
-// The cycle on the device commit.  slot[0] already holds the first batch.  Returns with handoff = true (and slot[0]
-// holding the next, not yet committed batch) when the rest of the cycle belongs to the host commit.
+// The cycle on the device commit.  slot[0] already holds the first batch.  Returns with handoff = true when the rest of
+// the cycle belongs to the host commit.
 int run_lattice(yk_engine* e, Cycle& c, bool& handoff) {
     handoff = false;
-    const bool ins = e->ord.insensitive;
-    Slot& A = e->slot[0];
-    size_t bsz = ins ? (size_t)e->maxA : (size_t)e->batch;
-    const size_t bmax = bsz;
     int rc = lt_prepare(e);
     if (rc) return rc;
-    bool first = true;
-    while (!A.asks.empty()) {
-        const size_t B = A.asks.size();
-        memcpy(e->h_lt_asks.p, A.asks.data(), 4 * B);
-        if (!e->lt_plan_ready) {
-            yklt::build_meta(e->cm.t, e->lt_shape_ids, e->a_sigid.data(), A.asks, e->h_lt_meta.p, e->h_lt_shp.p, e->h_lt_sig.p);
-            ykun::plan_segments(e->h_lt_meta.p, e->h_lt_shp.p, e->h_lt_sig.p, (int)B, e->un_min > 0 ? e->un_min : (int)B + 1, e->un_segs);
-        }
-        e->lt_plan_ready = false;
-        size_t consumed = 0;
-        int status = yklt::ST_DONE;
-        if (e->nlive == 0) {   // no nodes: nothing fits
-            c.result.assign(B, YK_NONE);
-            consumed = ins ? B : 1;
-            if (!ins && e->a_gang[A.asks[0]] != YK_NONE)
-                while (consumed < B && e->cm.same_gang(A.asks[0], A.asks[consumed])) ++consumed;
-            if (!ins) status = yklt::ST_STOPPED;
-        } else {
-            if (first) {   // the initial order's NaN flag (device_order) is checked before the first batch commits anything:
-                           // a failed cycle must leave the node tables as they were
-                CK(cudaStreamSynchronize(e->stream));
-                if (e->h_flag[0]) return e->fail(YK_ERR_RANGE, "NaN node score (zero total on a weighted resource)");
-            }
-            rc = lt_batch(e, B, ins);
-            if (rc) return rc;
-            status = e->h_lt_hdr[yklt::H_STATUS];
-            consumed = (size_t)e->h_lt_hdr[yklt::H_CONSUMED];
-            if (status == yklt::ST_NAN) return e->fail(YK_ERR_RANGE, "NaN node score after commit");
-            if (consumed > B) return e->fail(YK_ERR_CUDA, "lattice kernel returned a bad header");
-            c.result.assign(e->h_lt_res.p, e->h_lt_res.p + B);
-        }
-        first = false;
-        e->st.lattice_asks += consumed;
-        e->st.batches++;
-        bool failed = false;
-        if (status == yklt::ST_HANDOFF) {
-            e->ord.unfill(A.snap, A.asks, consumed);   // the undecided tail goes back to the orderer
-            bool f2 = false;
-            A.asks.resize(consumed);
-            c.result.resize(consumed);
-            settle(e, c, A, nullptr, false, consumed, true /* no failure cut: every decided entry stands */, f2);
-            // (settle with ins = true calls fail_in_place for NONE entries, which is what a placement-insensitive order
-            //  wants; a placement-sensitive batch never carries a NONE before a hand-over: the kernel stops there instead)
-            e->st.lattice_handoffs++;
-            handoff = true;
-            return YK_OK;
-        }
-        settle(e, c, A, nullptr, false, consumed, ins, failed);
-        if (!failed && consumed < B) return e->fail(YK_ERR_CUDA, "lattice kernel ended a batch early without a failure");
-        bsz = failed ? std::max<size_t>(std::min<size_t>(64, bmax), bsz / 4) : std::min<size_t>(bmax, bsz * 2);
-        rc = fill_batch(e, bsz, bmax, (size_t)c.max_bindings - c.n, A, e->st);
-        if (rc) return rc;
+    Slot& A = e->slot[0];
+    yklt::Loop lp{e->ord, e->cm.t, e->lt_shape_ids, e->a_sigid.data(), A.asks, A.snap, c.result,
+                  e->h_lt_meta.p, e->h_lt_shp.p, e->h_lt_sig.p, e->un_segs, e->lt_plan_ready, e->un_min, e->nlive == 0,
+                  e->ord.insensitive ? (size_t)e->maxA : (size_t)e->batch, c.max_bindings, c.n, e->st};
+    if (e->nlive && !A.asks.empty()) {   // the initial order's NaN flag (device_order) is checked before the first batch
+                                          // commits anything: a failed cycle must leave the node tables as they were
+        CK(cudaStreamSynchronize(e->stream));
+        if (e->h_flag[0]) return e->fail(YK_ERR_RANGE, "NaN node score (zero total on a weighted resource)");
     }
-    return YK_OK;
+    return yklt::device_commit(lp, [&](size_t B, int* status, size_t* consumed) { return lt_batch(e, B, status, consumed, c.result); },
+                               [&](uint32_t a, uint32_t node) { bind_one(e, c, a, node); },
+                               [&](int code, const char* m) { return e->fail(code, m); }, handoff);
 }
 
 // The cycle on the sweep + host commit path.  slot[0] holds the first batch (filled, not yet launched); the host commit's
@@ -1646,8 +1519,9 @@ int run_host(yk_engine* e, Cycle& c) {
         rc = commit(e, A, ins, c.result, consumed);
         if (forked) { e->worker.wait(); merge_worker_stats(); }
         if (rc) return rc;
-        bool failed = false;
-        settle(e, c, A, &Nx, forked, consumed, ins, failed);
+        // the speculated fill is undone even when it produced no batch: it may still have marked asks (headroom skips)
+        const bool failed = yk::settle(e->ord, A.asks, A.snap, forked ? &Nx.snap : nullptr, c.result.data(), consumed, ins, e->st,
+                                       [&](uint32_t a, uint32_t node) { bind_one(e, c, a, node); });
         if (rc_next) return rc_next;   // this batch's bindings stand; the speculated one never ran
         if (failed && Nx.B > 0) {   // the speculated batch was built on an order that did not happen: drop it
             rc = drain(e, Nx);
@@ -1655,8 +1529,7 @@ int run_host(yk_engine* e, Cycle& c) {
             Nx.asks.clear(); Nx.B = 0; Nx.nchunks = 0;
         }
         if (failed) { Nx.asks.clear(); Nx.B = 0; Nx.nchunks = 0; }
-        // after a failure in a placement-sensitive order, probe with short batches until placements resume
-        bsz = failed ? std::max<size_t>(std::min<size_t>(64, e->batch), bsz / 4) : std::min<size_t>(e->batch, bsz * 2);
+        bsz = yk::next_batch_size(bsz, bmax, failed);
         if (Nx.B == 0 && c.n < c.max_bindings) {
             // nothing in flight: the epoch may end here (merge order, refresh the device view) before the next batch
             if (e->cm.dirty_list.size() * 2 >= (size_t)e->epoch_limit || failed) {
@@ -1777,7 +1650,7 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
     e->st.host_ms[0] += t_a - t_start;
     e->st.host_ms[1] += begin_ms;
     if (rc) return rc;
-    if (gang_too_big) return e->fail(YK_ERR_ARG, "yk_cycle: a gang has more members than the sweep batch (raise yk_config.batch)");
+    if (gang_too_big) return e->fail(YK_ERR_ARG, yk::GANG_TOO_BIG);
 
     Cycle c;
     c.max_bindings = max_bindings; c.out = out;

@@ -104,7 +104,9 @@ typedef enum {
    (>= 2048 consecutive asks with one request vector and one predicate signature: the replicas of a deployment, the executors of
    a job, the reference's own benchmark) and that is eligible (fair node sort, non-negative weights and weighted totals, unique
    NodeID ranks, every gang's members requesting one vector) is decided on the device by a grid-wide sort (csrc/yk_uniform.cuh);
-   every other cycle takes the sweep + host commit path.  The bindings are the same either way. */
+   so is an eligible cycle of at least 10 000 pending asks without masks (no required / forbidden labels, no node name, every
+   node taint tolerated, no gangs) in a placement-insensitive order, by rounds at the front of the node order
+   (csrc/yk_rounds.cuh); every other cycle takes the sweep + host commit path.  The bindings are the same either way. */
 #define YK_FLAG_HOST_COMMIT 2u      /* never commit on the device */
 #define YK_FLAG_DEVICE_COMMIT 4u    /* commit on the device whenever the cycle is eligible, also where the order is not made of
                                       uniform runs (yk_lattice_kernel: exact, no bitmap read-back, no host work per ask, but
@@ -158,6 +160,9 @@ typedef struct {
     /* uniform runs of the device commit (consecutive asks with one request vector and one predicate signature, decided by a
        grid-wide sort instead of the sequential chain): runs, asks they decided, elements generated, deeper retries */
     uint64_t uniform_runs, uniform_asks, uniform_elements, uniform_retries;
+    /* round commit of the device commit (mask-free stretches decided in rounds at the front of the node order): passes
+       (rounds and single steps), asks it decided, single steps (the front node rejected the ask) */
+    uint64_t round_passes, round_asks, round_single_steps;
 } yk_stats_t;
 
 int yk_create(const yk_config* cfg, yk_engine** out);

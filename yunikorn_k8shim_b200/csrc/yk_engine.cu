@@ -30,6 +30,7 @@
 #include "yk_filter.cuh"
 #include "yk_lattice.cuh"
 #include "yk_uniform.cuh"
+#include "yk_rounds.cuh"
 #include "yk_commit.hpp"
 #include "yk_lattice_host.hpp"
 #include "yk_orderer.hpp"
@@ -42,6 +43,11 @@ namespace {
 constexpr int NPT = YK_NPT;       // sorted-node positions per sweep thread
 constexpr int AC = 128;           // asks per sweep CTA chunk
 constexpr int NODE_TILE = YK_SWEEP_THREADS * NPT;
+// round commit (yk_rounds.h), measured on H100 by scripts/round_prof.py (DESIGN.md §6.3): mask-free fair cycles of 10 000
+// asks and more are faster on it, 5 000 are not
+constexpr int RD_MIN = 10000;               // fewest pending asks for which a mask-free cycle starts on the device commit
+constexpr double RD_US_PER_ASK = 0.19;      // whole cycle per ask on the round commit (config 2: 8.7-10.1 ms / 50 000)
+constexpr double RD_HOST_US_PER_ASK = 0.28; // ... and on the sweep + host commit (config 2: 12.4-19.7 ms / 50 000)
 
 inline size_t round_up(size_t v, size_t m) { return (v + m - 1) / m * m; }
 
@@ -282,6 +288,14 @@ struct yk_engine {
     Dev<ykun::Globals> d_un_g; Pin<ykun::Globals> h_un_g;
     Dev<uint8_t> d_un_cub; size_t un_cub_bytes = 0;
     std::vector<ykun::Segment> un_segs;
+    // round commit (yk_rounds.h) of mask-free stretches, automatic commit only
+    int rd_min = RD_MIN;                        // fewest pending asks for which a mask-free cycle starts on it (YK_ROUND_MIN; 0: never)
+    int rd_window = ykrd::WCAP;                 // candidates per round (YK_ROUND_WINDOW: a testing knob)
+    int rd_guard = ykrd::GUARD;                  // asks per pass below which a stretch hands over to the host commit (YK_ROUND_GUARD)
+    uint64_t rd_taints = 0;                     // this cycle: union of the live nodes' taints
+    bool rd_maskfree = false;                   // this cycle: every pending ask is round-eligible (no gang, no masks)
+    size_t rd_smem = 0;
+    Dev<yklt::Ent> d_rd_spent; Dev<int> d_rd_hdr; Pin<int> h_rd_hdr;
     Dev<uint32_t> pre_q; Dev<int64_t> pre_v; Dev<int32_t> pre_o;   // yk_preemption_search staging, grown on demand
     // yk_filter_nodes: its own node order (so a cycle's sort buffers are never touched) and per-chunk buffers, grown on demand
     Dev<uint64_t> f_key_in, f_key_out; Dev<uint32_t> f_val_in, f_val_out; Dev<uint8_t> f_cub; size_t f_cub_bytes = 0;
@@ -334,6 +348,30 @@ void launch_lattice(int D, const yklt::Args& a, size_t smem, cudaStream_t s) {
         case 6: yk_lattice_kernel<6><<<1, yklt::THREADS, smem, s>>>(a); break;
         case 7: yk_lattice_kernel<7><<<1, yklt::THREADS, smem, s>>>(a); break;
         default: yk_lattice_kernel<8><<<1, yklt::THREADS, smem, s>>>(a); break;
+    }
+}
+template <int D>
+cudaError_t rounds_setup_d(size_t smem) {
+    return cudaFuncSetAttribute(yk_rounds_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+}
+cudaError_t rounds_setup(int D, size_t* smem) {
+    *smem = sizeof(ykrd::Shared);
+    switch (D) {
+        case 1: return rounds_setup_d<1>(*smem); case 2: return rounds_setup_d<2>(*smem); case 3: return rounds_setup_d<3>(*smem);
+        case 4: return rounds_setup_d<4>(*smem); case 5: return rounds_setup_d<5>(*smem); case 6: return rounds_setup_d<6>(*smem);
+        case 7: return rounds_setup_d<7>(*smem); default: return rounds_setup_d<8>(*smem);
+    }
+}
+void launch_rounds(int D, const ykrd::Args& a, size_t smem, cudaStream_t s) {
+    switch (D) {
+        case 1: yk_rounds_kernel<1><<<1, yklt::THREADS, smem, s>>>(a); break;
+        case 2: yk_rounds_kernel<2><<<1, yklt::THREADS, smem, s>>>(a); break;
+        case 3: yk_rounds_kernel<3><<<1, yklt::THREADS, smem, s>>>(a); break;
+        case 4: yk_rounds_kernel<4><<<1, yklt::THREADS, smem, s>>>(a); break;
+        case 5: yk_rounds_kernel<5><<<1, yklt::THREADS, smem, s>>>(a); break;
+        case 6: yk_rounds_kernel<6><<<1, yklt::THREADS, smem, s>>>(a); break;
+        case 7: yk_rounds_kernel<7><<<1, yklt::THREADS, smem, s>>>(a); break;
+        default: yk_rounds_kernel<8><<<1, yklt::THREADS, smem, s>>>(a); break;
     }
 }
 
@@ -625,12 +663,45 @@ int lt_window(yk_engine* e, size_t off, size_t B) {
     return YK_OK;
 }
 
+// One round-eligible stretch [off, off + B) of the staged batch through yk_rounds_kernel.
+int lt_rounds(yk_engine* e, size_t off, size_t B, int* status, size_t* consumed) {
+    cudaStream_t s = e->stream;
+    { const int rco = un_reorder(e); if (rco) return rco; }
+    ykrd::Args a{};
+    a.policy = e->cfg.policy;
+    for (int k = 0; k < 8; ++k) a.w[k] = e->w.w[k];
+    a.rec = e->d_rec.p; a.RS = e->lt_RS; a.ord[0] = e->d_ord[0].p; a.ord[1] = e->d_ord[1].p; a.cur = e->d_lt_cur.p;
+    a.nlive = (int)e->nlive; a.spent = e->d_rd_spent.p;
+    a.a_req = e->d_areq.p; a.lda = e->maxA; a.a_tol = e->d_atol.p; a.a_need = e->d_aneed.p; a.a_deny = e->d_adeny.p; a.a_node = e->d_anode.p;
+    a.asks = e->d_lt_asks.p + off; a.B = (int)B; a.res = e->d_lt_res.p + off; a.hdr = e->d_rd_hdr.p;
+    a.window = std::max(1, std::min(e->rd_window, ykrd::WCAP)); a.guard = e->rd_guard;
+    a.prof = e->lt_prof ? e->d_lt_prof.p + 16 : nullptr;
+    CK(cudaEventRecord(e->ev_l0, s));
+    launch_rounds(e->D, a, e->rd_smem, s);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(e->ev_l1, s));
+    CK(cudaMemcpyAsync(e->h_rd_hdr.p, e->d_rd_hdr.p, ykrd::R_WORDS * sizeof(int), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, e->ev_l0, e->ev_l1);
+    e->st.lattice_ms += ms;
+    e->st.lattice_launches += 1;
+    e->st.d2h_bytes += ykrd::R_WORDS * sizeof(int);
+    const int* h = e->h_rd_hdr.p;
+    *status = h[ykrd::R_STATUS];
+    *consumed = (size_t)h[ykrd::R_CONSUMED];
+    if (*consumed > B) return e->fail(YK_ERR_CUDA, "round kernel returned a bad header");
+    e->st.round_passes += (uint64_t)h[ykrd::R_PASSES]; e->st.round_single_steps += (uint64_t)h[ykrd::R_SINGLES];
+    e->st.round_asks += *consumed;
+    return YK_OK;
+}
+
 // One batch of slot[0] (segments planned in e->un_segs) through yklt::run_segments; the decided entries' nodes land in
 // `result`.  Blocks until it is decided.
 int lt_batch(yk_engine* e, size_t B, int* status, size_t* done, std::vector<uint32_t>& result) {
     cudaStream_t s = e->stream;
     memcpy(e->h_lt_asks.p, e->slot[0].asks.data(), 4 * B);
-    bool staged = false;   // only the windowed kernel reads the per-entry words
+    bool staged = false, asks_staged = false;   // only the windowed kernel reads the per-entry words, the round kernel the asks
     auto uniform = [&](size_t off, size_t len, bool has_gang, int* ust, size_t* consumed) { return lt_uniform(e, off, len, has_gang, ust, consumed); };
     auto window = [&](size_t off, size_t len, int* st, size_t* consumed) -> int {
         if (!staged) {
@@ -639,7 +710,7 @@ int lt_batch(yk_engine* e, size_t B, int* status, size_t* done, std::vector<uint
             CK(cudaMemcpyAsync(e->d_lt_shp.p, e->h_lt_shp.p, 4 * B, cudaMemcpyHostToDevice, s));
             CK(cudaMemcpyAsync(e->d_lt_sig.p, e->h_lt_sig.p, 4 * B, cudaMemcpyHostToDevice, s));
             e->st.h2d_bytes += 16 * B;
-            staged = true;
+            staged = asks_staged = true;
         }
         const int rc = lt_window(e, off, len);
         if (rc) return rc;
@@ -648,7 +719,17 @@ int lt_batch(yk_engine* e, size_t B, int* status, size_t* done, std::vector<uint
         if (*consumed > len) return e->fail(YK_ERR_CUDA, "lattice kernel returned a bad header");
         return YK_OK;
     };
-    const int rc = yklt::run_segments(e->un_segs, e->h_lt_meta.p, uniform, window, status, done);
+    // the round commit takes the mask-free stretches of an automatic cycle; it reads the asks only
+    auto rounds = [&](size_t off, size_t len, int* st, size_t* consumed) -> int {
+        if (!asks_staged) {
+            CK(cudaMemcpyAsync(e->d_lt_asks.p, e->h_lt_asks.p, 4 * B, cudaMemcpyHostToDevice, s));
+            e->st.h2d_bytes += 4 * B;
+            asks_staged = true;
+        }
+        return lt_rounds(e, off, len, st, consumed);
+    };
+    auto stretch = yklt::route_stretches(!e->lt_force, e->cm.t, e->ord.insensitive, e->rd_taints, e->h_lt_asks.p, rounds, window);
+    const int rc = yklt::run_segments(e->un_segs, e->h_lt_meta.p, uniform, stretch, status, done);
     if (rc) return rc;
     if (*done) {
         CK(cudaMemcpyAsync(e->h_lt_res.p, e->d_lt_res.p, 4 * *done, cudaMemcpyDeviceToHost, s));
@@ -1014,11 +1095,15 @@ void yk_destroy(yk_engine* e) {
                         "run %.3f  epoch end / export + sync %.3f  finish %.3f\n", (unsigned long long)e->hp_n, e->hp[0] / e->hp_n, e->hp[1] / e->hp_n,
                 e->hp[2] / e->hp_n, e->hp[3] / e->hp_n, e->hp[4] / e->hp_n, e->hp[5] / e->hp_n, e->hp[6] / e->hp_n);
     if (e->lt_prof && e->d_lt_prof.p) {
-        long long pf[16] = {0};
+        long long pf[32] = {0};
         if (cudaMemcpy(pf, e->d_lt_prof.p, sizeof(pf), cudaMemcpyDeviceToHost) == cudaSuccess) {
             static const char* nm[yklt::PF_N] = {"stage", "scan", "window", "bound", "lattice", "sort", "links+rows", "chain", "apply", "patch", "fullscan"};
             fprintf(stderr, "[ykgpu] lattice kernel, SM clocks per phase (%llu sub-runs):", (unsigned long long)e->lt_total_subruns);
             for (int k = 0; k < yklt::PF_N; ++k) fprintf(stderr, " %s=%lld", nm[k], pf[k]);
+            fprintf(stderr, "\n");
+            static const char* rn[ykrd::RP_N] = {"stretch_edges", "candidates", "prefix_min", "apply", "sort", "merge", "single_steps"};
+            fprintf(stderr, "[ykgpu] round kernel, SM clocks per phase (%llu passes):", (unsigned long long)e->st.round_passes);
+            for (int k = 0; k < ykrd::RP_N; ++k) fprintf(stderr, " %s=%lld", rn[k], pf[16 + k]);
             fprintf(stderr, "\n");
         }
     }
@@ -1124,9 +1209,14 @@ int yk_create(const yk_config* cfg, yk_engine** out) {
     e->hp_on = getenv("YK_PROFILE_HOST") != nullptr;
     if (const char* um = getenv("YK_UNIFORM_MIN")) e->un_min = atoi(um);   // 0: no uniform-run path
     if (const char* ud = getenv("YK_UNIFORM_DEPTH")) e->un_depth = std::max(0, atoi(ud));   // 0 / unset: the engine's own rule
-    T(e->d_lt_prof.alloc(16));
-    if (ok) T(cudaMemset(e->d_lt_prof.p, 0, 16 * sizeof(long long)));
+    if (const char* rm = getenv("YK_ROUND_MIN")) e->rd_min = std::max(0, atoi(rm));         // 0: no cycle starts on the round commit
+    if (const char* rw = getenv("YK_ROUND_WINDOW")) e->rd_window = std::max(1, std::min(atoi(rw), ykrd::WCAP));
+    if (const char* rg = getenv("YK_ROUND_GUARD")) e->rd_guard = std::max(0, atoi(rg));
+    T(e->d_rd_spent.alloc(N)); T(e->d_rd_hdr.alloc(ykrd::R_WORDS)); T(e->h_rd_hdr.alloc(ykrd::R_WORDS));
+    T(e->d_lt_prof.alloc(32));   // [0, 16) the lattice kernel's phases, [16, 32) the round kernel's
+    if (ok) T(cudaMemset(e->d_lt_prof.p, 0, 32 * sizeof(long long)));
     if (ok) T(lattice_setup(D, &e->lt_smem));
+    if (ok) T(rounds_setup(D, &e->rd_smem));
     T(e->h_snode.alloc(N)); T(e->h_skey.alloc(N));
     T(e->h_dirty_nodes.alloc(N)); T(e->h_dirty_vals.alloc(N * D)); T(e->h_flag.alloc(1)); T(e->h_scores.alloc(N));
     if (ok) {   // does this binary carry an image the device can run?
@@ -1578,6 +1668,10 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
         // (longest run of one signature id among consecutive pending asks, in index order: the hint for the automatic commit choice)
         size_t sig_run = 0, sig_longest = 0;
         uint32_t sig_prev = YK_NONE;
+        // (and whether every pending ask is free of masks -- yklt::round_eligible -- for the round commit)
+        uint64_t taints = 0;
+        if (auto_lattice) for (uint32_t n = 0; n < e->n_hi; ++n) if (e->n_present[n]) taints |= e->n_taint[n];
+        bool maskfree = auto_lattice;
         for (uint32_t a = 0; a < e->a_hi; ++a) {
             uint8_t& st = e->a_state[a];
             if (st == yk::ST_ABSENT || st == yk::ST_ALLOCATED) continue;
@@ -1588,10 +1682,13 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
             if (auto_lattice) {
                 const uint32_t g = e->a_sigid[a];
                 if (g == sig_prev) ++sig_run; else { sig_longest = std::max(sig_longest, sig_run); sig_run = 1; sig_prev = g; }
+                maskfree = maskfree && e->a_need[a] == 0 && e->a_deny[a] == 0 && e->a_node[a] == YK_NONE && (taints & ~e->a_tol[a]) == 0;
             }
         }
         sig_longest = std::max(sig_longest, sig_run);
         e->cycle_has_gang = any_gang;
+        e->rd_taints = taints;
+        e->rd_maskfree = maskfree && !any_gang;
         if (any_gang) {   // a gang that no batch can hold is an argument error: found before anything is committed
             std::unordered_map<uint64_t, uint32_t> members;
             for (uint32_t a : pending)
@@ -1630,7 +1727,9 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
         }
         // a hint only (it sizes the first batch, never decides): asks are usually upserted application by application, so a long
         // run of one signature in index order promises one in the orderer's order
-        e->un_hint = !gang_too_big && auto_lattice && pending.size() >= (size_t)e->un_min && sig_longest >= (size_t)e->un_min;
+        e->un_hint = !gang_too_big && auto_lattice &&
+                     ((pending.size() >= (size_t)e->un_min && sig_longest >= (size_t)e->un_min) ||
+                      (e->rd_maskfree && e->rd_min > 0 && pending.size() >= (size_t)e->rd_min));
         if (!gang_too_big && force_lattice) {   // request-vector numbers for the lattice kernel's windows
             yklt::assign_shapes(e->cm.t, pending, e->a_shape, &e->n_shapes);
             e->lt_shape_ids = e->a_shape.data();
@@ -1666,11 +1765,14 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
     if (auto_lattice && e->un_hint && ins) bsz0 = e->maxA;
     e->lt_plan_ready = false;
     rc = fill_batch(e, bsz0, std::max<size_t>(bsz0, e->batch), max_bindings, e->slot[0], e->st);
-    if (!rc && auto_lattice && pending.size() >= (size_t)e->un_min && e->slot[0].asks.size() >= (size_t)e->un_min) {
+    // a big mask-free cycle in a placement-insensitive order: its stretches between uniform runs go to the round commit
+    const bool round_screen = ins && e->rd_maskfree && e->rd_min > 0 && pending.size() >= (size_t)e->rd_min;
+    if (!rc && auto_lattice && ((pending.size() >= (size_t)e->un_min && e->slot[0].asks.size() >= (size_t)e->un_min) || round_screen)) {
         // Automatic: the device commit decides a uniform run (one request vector, one predicate signature) by a grid-wide sort,
-        // everything else through a sequential chain that one host core still does faster (DESIGN.md §6.2).  So the
-        // cycle starts on the device exactly when the order is made of long uniform runs.  Cheap screen first -- the
-        // longest run of one signature id in the first batch -- and only then the eligibility test and the shape numbers.
+        // a mask-free stretch by rounds at the front of the node order (DESIGN.md §6.3), everything else through a
+        // sequential chain that one host core still does faster (DESIGN.md §6.2).  So the cycle starts on the device when
+        // its order is made of long uniform runs or when it is big and mask-free.  Cheap screens first -- the longest run
+        // of one signature id in the first batch, the pending scan's mask-free flag -- and only then the eligibility test.
         const std::vector<uint32_t>& as = e->slot[0].asks;
         size_t longest = 0, run = 1;
         for (size_t i = 1; i <= as.size(); ++i) {
@@ -1678,7 +1780,7 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
             longest = std::max(longest, run);
             run = 1;
         }
-        if (longest >= (size_t)e->un_min) {
+        if (longest >= (size_t)e->un_min || round_screen) {
             const yklt::Eligibility el = yklt::eligible(e->cm.t, e->n_hi, e->n_present.data(), e->n_total.p, e->maxN, e->n_rank.data(), pending, &e->ranks_unique, &e->cycle_has_gang);
             if (el.ok) {
                 // signature ids double as shape numbers: equal signatures request equal vectors; two signatures with one request
@@ -1695,9 +1797,15 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
                     ykun::plan_segments(e->h_lt_meta.p, e->h_lt_shp.p, e->h_lt_sig.p, (int)B0, e->un_min, e->un_segs);
                     // measured costs (H100, bench.py device_commit / host_commit arms): a uniform run ~0.2-0.3 ms whatever its
                     // length (16 launches, one round trip), a windowed ask ~0.35 us, an ask on the host commit ~0.08-0.13 us
-                    double dev_us = 0;
-                    for (const ykun::Segment& sg : e->un_segs) dev_us += sg.uniform ? 250.0 : 0.35 * sg.len;
-                    lattice = dev_us < 0.7 * 0.08 * (double)B0;
+                    // (the host side gets a 30 % margin); a round stretch is priced in whole-cycle time per ask on both sides
+                    // (scripts/round_prof.py), which is how it was measured
+                    double dev_us = 0, host_us = 0;
+                    for (const ykun::Segment& sg : e->un_segs) {
+                        const bool rounds = !sg.uniform && yklt::round_eligible(e->cm.t, ins, e->rd_taints, e->slot[0].asks.data() + sg.off, (size_t)sg.len);
+                        dev_us += sg.uniform ? 250.0 : (rounds ? RD_US_PER_ASK : 0.35) * sg.len;
+                        host_us += (rounds ? RD_HOST_US_PER_ASK : 0.7 * 0.08) * sg.len;
+                    }
+                    lattice = dev_us < host_us;
                     e->lt_plan_ready = lattice;
                 }
             }

@@ -289,6 +289,29 @@ inline int run_segments(const std::vector<ykun::Segment>& segs, const uint32_t* 
     return 0;
 }
 
+// Whether the round commit (yk_rounds.h) may decide a stretch of asks: a placement-insensitive order (a NOFIT fails in
+// place), no gang member, and no masks -- no required or forbidden labels, no node name, every taint of the live nodes
+// (`taints`, their union) tolerated.
+inline bool round_eligible(const yk::CommitTables& t, bool insensitive, uint64_t taints, const uint32_t* asks, size_t len) {
+    if (!insensitive) return false;
+    for (size_t i = 0; i < len; ++i) {
+        const uint32_t a = asks[i];
+        if (t.a_gang[a] != yk::CNONE || t.a_need[a] || t.a_deny[a] || t.a_node[a] != yk::CNONE || (taints & ~t.a_tol[a])) return false;
+    }
+    return true;
+}
+
+// The window callback of run_segments for a cycle on the device commit: a round-eligible stretch goes through
+// rounds(off, len, &status, &consumed) when `rounds_on`, every other one through window(...).
+template <class Rounds, class Window>
+inline auto route_stretches(bool rounds_on, const yk::CommitTables& t, bool insensitive, uint64_t taints, const uint32_t* asks,
+                            Rounds& rounds, Window& window) {
+    return [=, &t, &rounds, &window](size_t off, size_t len, int* status, size_t* consumed) -> int {
+        if (rounds_on && round_eligible(t, insensitive, taints, asks + off, len)) return rounds(off, len, status, consumed);
+        return window(off, len, status, consumed);
+    };
+}
+
 // What the device commit's batch loop works on; the caller owns all of it.
 struct Loop {
     yk::Orderer& ord;

@@ -991,6 +991,47 @@ func (e *Engine) pageNames(page []C.uint32_t) []string {
 	return names
 }
 
+// PreemptionNodes: the search half of a preemptor (PreemptionPredicates, predicate_manager.go:137-175, for every node at
+// once).  victimKeys are the allocations the caller's preemption policy lets go for askKey, in its victim order; the engine
+// knows where each is bound.  Returns the nodes where removing a prefix of those victims (in that order, per node) lets the
+// ask fit, fit ranks skip .. skip+k-1 in the engine's node order, with the number of victims each needs, then how many
+// nodes fit in all and the one needing the fewest (empty name when none fits).  Which allocations may be victims, and
+// releasing them, stay with the caller.
+func (e *Engine) PreemptionNodes(askKey string, victimKeys []string, skip, k uint32) (nodes []string, need []uint32, nFit uint32, best string, bestNeed uint32, err error) {
+	e.mu.Lock()
+	defer e.mu.Unlock()
+	a, ok := e.askIdx[askKey]
+	if !ok {
+		return nil, nil, 0, "", 0, fmt.Errorf("ykgpu: unknown ask %s", askKey)
+	}
+	vic := make([]C.uint32_t, len(victimKeys)+1) // one spare element so &vic[0] is valid for an empty list
+	for i, key := range victimKeys {
+		v, ok := e.askIdx[key]
+		if !ok {
+			return nil, nil, 0, "", 0, fmt.Errorf("ykgpu: unknown victim %s", key)
+		}
+		vic[i] = C.uint32_t(v)
+	}
+	off := [2]C.uint32_t{0, C.uint32_t(len(victimKeys))}
+	page := make([]C.uint32_t, k+1)
+	cnt := make([]C.uint32_t, k+1)
+	var fit, bn, bc C.uint32_t
+	i := C.uint32_t(a)
+	if err := e.ck(C.yk_preemption_nodes(e.h, 1, &i, &off[0], &vic[0], C.uint32_t(skip), C.uint32_t(k), &page[0], &cnt[0], &fit,
+		&bn, &bc), "yk_preemption_nodes"); err != nil {
+		return nil, nil, 0, "", 0, err
+	}
+	nodes = e.pageNames(page[:k])
+	need = make([]uint32, len(nodes))
+	for j := range need {
+		need[j] = uint32(cnt[j])
+	}
+	if bn != C.YK_NONE {
+		best = e.nodes[bn].name
+	}
+	return nodes, need, uint32(fit), best, uint32(bc), nil
+}
+
 // slowPath: pods whose predicates do not reduce to the bit sets.  Candidates are tried in the engine's node order
 // (ascending float64 score, then NodeID) through the UNCHANGED Go path -- callback.Predicates ->
 // Context.IsPodFitNode -> PredicateManager (scheduler_callback.go:196-198) -- and the first node that passes is pinned:

@@ -33,6 +33,9 @@
  *   yk_filter_nodes                     the same answers for every node and a list of asks at once: the candidates a
  *                                       slow-path pod is walked through Predicates in, and the per-cause counts of the
  *                                       FAILED reason of an unplaceable pod
+ *   yk_preemption_search                ResourceManagerCallback.PreemptionPredicates for one (ask, node, victims) query
+ *   yk_preemption_nodes                 the same search on every node for a list of asks, from the allocations the
+ *                                       engine made: the search half of a preemptor (its policy stays with the caller)
  *
  * Conventions: every call returns YK_OK (0) or a negative yk_status; no exceptions or aborts cross the
  * boundary.  Inputs are caller-owned host memory, fully consumed before return (cgo: no Go pointer is
@@ -275,6 +278,39 @@ int yk_filter_nodes(yk_engine* e, uint32_t n, const uint32_t* asks, int allocate
  * each victim gives back to the node.  Known answers: TestPreemptionPredicates(+Empty), predicate_manager_test.go:67-134. */
 int yk_preemption_search(yk_engine* e, uint32_t n_queries, const uint32_t* ask, const uint32_t* node,
                          const uint32_t* victim_off, const int64_t* victim_req, const uint32_t* start, int32_t* index_out);
+
+/* The same victim search over every node at once, for allocations this engine made: for each ask a victim list (the
+ * caller's policy picks the victims and their order), and back the nodes those victims can free, in the cycle's node order,
+ * evaluated on the device (csrc/yk_preempt_nodes.cuh).  The engine knows where each victim is bound and what it holds, so
+ * the caller sends only ask indices.  Read-only.
+ *   Victims of ask i on node p: V(i,p) = the entries of victims[victim_off[i] .. victim_off[i+1]) bound to p, in list order.
+ *     answer(i,p) is exactly what yk_preemption_search(asks[i], p, <requests of V(i,p)>, start = 0) returns on the current
+ *     tables.  p FITS when answer >= 0 and then needs answer + 1 victims.  A node with no victim in the list does not fit (the
+ *     reference's loop never runs for it).  Reservation flags are not consulted (PreemptionPredicates does not look at
+ *     them); an unschedulable node fails the static part.
+ *   Nodes considered: every present node, ordered as yk_filter_nodes orders them (ascending float64 score, then name_rank,
+ *     then index).  An entry whose victim is bound to a node that is no longer present is ignored.
+ *   Per ask: n_fit[i] = the number of fitting nodes; nodes_out[i*k + j] / need_out[i*k + j] = the fitting node of fit rank
+ *     skip + j and its victim count (YK_NONE / 0 past the last one); best_node[i] / best_need[i] = the fitting node with the
+ *     fewest victims, ties to the earlier node in the order (YK_NONE / 0 when nothing fits).  An ask that is not present has
+ *     no fitting node.
+ *   Errors, all checked before any device work; nothing is written on an error:
+ *     YK_ERR_ARG   asks / victim_off NULL with n > 0, victims NULL with victim_off[n] > 0, nodes_out NULL with k > 0, an ask
+ *                  or victim index >= max_asks, victim_off[0] != 0 or decreasing, the same victim twice in one list;
+ *     YK_ERR_STATE a victim that is not YK_ST_ALLOCATED;
+ *     YK_ERR_RANGE a present node scores NaN (as yk_cycle).
+ *     n == 0 is YK_OK.
+ *   No state changes: the next yk_cycle is the same whether or not this ran.  Counted in other_launches / h2d_bytes /
+ *     d2h_bytes; local to this engine whatever rank / world are.  Lists are processed in chunks of whole lists: a chunk ends
+ *     before the list that would take it past 4096 lists or 2^18 entries (a longer list is a chunk of its own). */
+int yk_preemption_nodes(yk_engine* e, uint32_t n, const uint32_t* asks,
+                        const uint32_t* victim_off /* [n+1], victim_off[0] = 0, non-decreasing */,
+                        const uint32_t* victims /* [victim_off[n]] ask indices, per ask in the caller's victim order */,
+                        uint32_t skip, uint32_t k,
+                        uint32_t* nodes_out /* [n][k] row-major, YK_NONE padded; may be NULL iff k == 0 */,
+                        uint32_t* need_out /* [n][k] victims needed on that node, 0 padded; may be NULL */,
+                        uint32_t* n_fit /* [n], may be NULL */,
+                        uint32_t* best_node /* [n], may be NULL */, uint32_t* best_need /* [n], may be NULL */);
 
 /* multi-GPU exchange hook: called once per batch on every rank, after the local shard's rows of `buf`
  * (device pointer, row-major, `row_bytes` per ask, rows [first_row, first_row+n_rows) are this rank's)

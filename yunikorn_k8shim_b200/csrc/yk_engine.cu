@@ -10,6 +10,7 @@
 #include "../../include/ykgpu.h"
 
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -28,6 +29,7 @@
 
 #include "yk_kernels.cuh"
 #include "yk_filter.cuh"
+#include "yk_preempt_nodes.cuh"
 #include "yk_lattice.cuh"
 #include "yk_uniform.cuh"
 #include "yk_rounds.cuh"
@@ -302,6 +304,12 @@ struct yk_engine {
     Dev<int> f_flag; Pin<int> h_f_flag;
     Dev<uint32_t> f_asks, f_bits, f_tcnt, f_counts, f_out;
     Pin<uint32_t> h_f_asks, h_f_counts, h_f_out;
+    // yk_preemption_nodes: node positions, per-chunk entry / group buffers and staging, grown on demand; pn_seen / pn_stamp find
+    // a victim named twice in one list
+    Dev<uint32_t> pn_pos, pn_in, pn_val_in, pn_val_out, pn_head, pn_incl, pn_gask, pn_gnode, pn_goff, pn_start, pn_out;
+    Dev<uint64_t> pn_key_in, pn_key_out; Dev<int64_t> pn_vreq; Dev<int32_t> pn_res; Dev<uint8_t> pn_cub;
+    Pin<uint32_t> h_pn_in, h_pn_out;
+    std::vector<uint32_t> pn_seen; uint32_t pn_stamp = 0;
     yk_allgather_fn xfn = nullptr; void* xctx = nullptr;
     // peer-to-peer exchange (see yk_peer_export): peers' slot buffers and sync blocks, mapped through CUDA IPC
     bool p2p = false;
@@ -1891,6 +1899,9 @@ namespace {
 constexpr uint32_t FILTER_CHUNK = 4096;      // asks per yk_filter_kernel launch at most
 constexpr size_t FILTER_WORDS = 1u << 24;    // device words per chunk at most (bitmap + tile counts + counts + window)
 constexpr int FILTER_AC = 32;                // asks per shared-memory stage of yk_filter_kernel
+constexpr uint32_t PN_ROWS = 4096;           // victim lists per yk_preemption_nodes chunk at most
+constexpr uint32_t PN_ENTRIES = 1u << 18;    // victim entries per chunk at most, unless one list alone is longer
+constexpr size_t PN_WORDS = 1u << 24;        // read-back words per chunk at most ([lists][2k + 3])
 
 void launch_filter(int D, const YkFilterArgs& a, dim3 grid, cudaStream_t s) {
     switch (D) {
@@ -1909,6 +1920,32 @@ template <typename T>
 cudaError_t grow(Dev<T>& d, size_t n) { return d.n < n ? d.alloc(n) : cudaSuccess; }
 template <typename T>
 cudaError_t grow(Pin<T>& h, size_t n) { return h.n < n ? h.alloc(n) : cudaSuccess; }
+
+// Enqueue the cycle's node order at this moment (ascending (score, NodeID rank, index)) into f_val_out[0, nlive), with the NaN
+// flag copied to h_f_flag (valid after the stream's next synchronise).  yk_filter_nodes and yk_preemption_nodes use it; its
+// buffers are their own, so a cycle's sort buffers are never touched.  Needs e->nlive > 0 and the tables uploaded.
+int filter_order(yk_engine* e) {
+    cudaStream_t s = e->stream;
+    const size_t N = e->maxN;
+    const uint32_t nlive = e->nlive;
+    if (e->f_key_in.n < N) {
+        CK(e->f_key_in.alloc(N)); CK(e->f_key_out.alloc(N)); CK(e->f_val_in.alloc(N)); CK(e->f_val_out.alloc(N));
+        size_t tb = 0;
+        CK(cub::DeviceRadixSort::SortPairs(nullptr, tb, e->f_key_in.p, e->f_key_out.p, e->f_val_in.p, e->f_val_out.p, (int)N, 0, 64, s));
+        e->f_cub_bytes = tb;
+        CK(e->f_cub.alloc(tb));
+        CK(e->f_flag.alloc(1)); CK(e->h_f_flag.alloc(1));
+    }
+    CK(cudaMemsetAsync(e->f_flag.p, 0, sizeof(int), s));
+    yk_key_kernel<<<(nlive + 255) / 256, 256, 0, s>>>(e->D, e->cfg.policy, e->w, e->d_total.p, e->d_avail.p, e->maxN, e->d_by_rank.p,
+                                                      (int)nlive, e->f_key_in.p, e->f_val_in.p, e->f_flag.p);
+    size_t tb = e->f_cub_bytes;
+    CK(cub::DeviceRadixSort::SortPairs(e->f_cub.p, tb, e->f_key_in.p, e->f_key_out.p, e->f_val_in.p, e->f_val_out.p, (int)nlive, 0, 64, s));
+    CK(cudaMemcpyAsync(e->h_f_flag.p, e->f_flag.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+    e->st.other_launches += 11;   // key + cub radix sort, as device_order
+    e->st.d2h_bytes += 4;
+    return YK_OK;
+}
 
 }  // namespace
 
@@ -2041,29 +2078,12 @@ int yk_filter_nodes(yk_engine* e, uint32_t n, const uint32_t* asks, int allocate
     const size_t row_words = (size_t)W + tiles + YK_FILTER_SLOTS + k;
     const uint32_t chunk = (uint32_t)std::min<size_t>({(size_t)n, FILTER_CHUNK, std::max<size_t>(1, FILTER_WORDS / row_words)});
     // device buffers are kept between calls and only grow
-    const size_t N = e->maxN;
-    if (e->f_key_in.n < N) {
-        CK(e->f_key_in.alloc(N)); CK(e->f_key_out.alloc(N)); CK(e->f_val_in.alloc(N)); CK(e->f_val_out.alloc(N));
-        size_t tb = 0;
-        CK(cub::DeviceRadixSort::SortPairs(nullptr, tb, e->f_key_in.p, e->f_key_out.p, e->f_val_in.p, e->f_val_out.p, (int)N, 0, 64, s));
-        e->f_cub_bytes = tb;
-        CK(e->f_cub.alloc(tb));
-        CK(e->f_flag.alloc(1)); CK(e->h_f_flag.alloc(1));
-    }
     CK(grow(e->f_asks, chunk)); CK(grow(e->h_f_asks, chunk));
     CK(grow(e->f_bits, (size_t)chunk * W)); CK(grow(e->f_tcnt, (size_t)chunk * tiles));
     CK(grow(e->f_counts, (size_t)chunk * YK_FILTER_SLOTS)); CK(grow(e->h_f_counts, (size_t)chunk * YK_FILTER_SLOTS));
     if (k) { CK(grow(e->f_out, (size_t)chunk * k)); CK(grow(e->h_f_out, (size_t)chunk * k)); }
-
-    // the cycle's node order at this moment: ascending (score, NodeID rank, index), with the NaN flag
-    CK(cudaMemsetAsync(e->f_flag.p, 0, sizeof(int), s));
-    yk_key_kernel<<<(nlive + 255) / 256, 256, 0, s>>>(D, e->cfg.policy, e->w, e->d_total.p, e->d_avail.p, e->maxN, e->d_by_rank.p,
-                                                      (int)nlive, e->f_key_in.p, e->f_val_in.p, e->f_flag.p);
-    size_t tb = e->f_cub_bytes;
-    CK(cub::DeviceRadixSort::SortPairs(e->f_cub.p, tb, e->f_key_in.p, e->f_key_out.p, e->f_val_in.p, e->f_val_out.p, (int)nlive, 0, 64, s));
-    CK(cudaMemcpyAsync(e->h_f_flag.p, e->f_flag.p, sizeof(int), cudaMemcpyDeviceToHost, s));
-    e->st.other_launches += 11;   // key + cub radix sort, as device_order
-    e->st.d2h_bytes += 4;
+    rc = filter_order(e);
+    if (rc) return rc;
 
     YkFilterArgs a{};
     a.total = e->d_total.p; a.avail = e->d_avail.p; a.ldn = e->maxN;
@@ -2105,6 +2125,145 @@ int yk_filter_nodes(yk_engine* e, uint32_t n, const uint32_t* asks, int allocate
         if (k) memcpy(nodes_out + (size_t)c0 * k, e->h_f_out.p, 4 * (size_t)rows * k);
         if (counts) memcpy(counts + (size_t)c0 * YK_FILTER_SLOTS, e->h_f_counts.p, 4 * (size_t)rows * YK_FILTER_SLOTS);
         if (n_pass) for (uint32_t i = 0; i < rows; ++i) n_pass[c0 + i] = e->h_f_counts[(size_t)i * YK_FILTER_SLOTS];
+    }
+    return YK_OK;
+}
+
+int yk_preemption_nodes(yk_engine* e, uint32_t n, const uint32_t* asks, const uint32_t* victim_off, const uint32_t* victims,
+                        uint32_t skip, uint32_t k, uint32_t* nodes_out, uint32_t* need_out, uint32_t* n_fit,
+                        uint32_t* best_node, uint32_t* best_need) {
+    if (!e) return YK_ERR_ARG;
+    std::lock_guard<std::mutex> g(e->mu);
+    if (n && (!asks || !victim_off)) return e->fail(YK_ERR_ARG, "yk_preemption_nodes: null asks or victim_off");
+    if (k && !nodes_out) return e->fail(YK_ERR_ARG, "yk_preemption_nodes: null nodes_out with k > 0");
+    if (!n) return YK_OK;
+    if (victim_off[0] != 0) return e->fail(YK_ERR_ARG, "yk_preemption_nodes: victim_off[0] must be 0");
+    for (uint32_t i = 0; i < n; ++i) {
+        if (asks[i] >= e->maxA) return e->fail(YK_ERR_ARG, "yk_preemption_nodes: ask index beyond max_asks");
+        if (victim_off[i] > victim_off[i + 1]) return e->fail(YK_ERR_ARG, "yk_preemption_nodes: victim_off must be non-decreasing");
+    }
+    const uint32_t nv = victim_off[n];
+    if (nv && !victims) return e->fail(YK_ERR_ARG, "yk_preemption_nodes: null victims");
+    if (e->pn_seen.size() < e->maxA) { e->pn_seen.assign(e->maxA, 0); e->pn_stamp = 0; }
+    for (uint32_t i = 0; i < n; ++i) {
+        if (++e->pn_stamp == 0) { std::fill(e->pn_seen.begin(), e->pn_seen.end(), 0u); e->pn_stamp = 1; }
+        for (uint32_t j = victim_off[i]; j < victim_off[i + 1]; ++j) {
+            const uint32_t v = victims[j];
+            if (v >= e->maxA) return e->fail(YK_ERR_ARG, "yk_preemption_nodes: victim index beyond max_asks");
+            if (e->pn_seen[v] == e->pn_stamp) return e->fail(YK_ERR_ARG, "yk_preemption_nodes: the same victim twice in one list");
+            e->pn_seen[v] = e->pn_stamp;
+        }
+    }
+    for (uint32_t j = 0; j < nv; ++j)
+        if (e->a_state[victims[j]] != yk::ST_ALLOCATED) return e->fail(YK_ERR_STATE, "yk_preemption_nodes: a victim holds no allocation");
+    int rc = upload_tables(e);
+    if (rc) return rc;
+    const uint32_t nlive = e->nlive;
+    auto write_empty = [&](uint32_t i0, uint32_t i1) {   // asks i0 .. i1-1 have no fitting node
+        if (k) std::fill(nodes_out + (size_t)i0 * k, nodes_out + (size_t)i1 * k, YK_NONE);
+        if (k && need_out) std::fill(need_out + (size_t)i0 * k, need_out + (size_t)i1 * k, 0u);
+        if (n_fit) std::fill(n_fit + i0, n_fit + i1, 0u);
+        if (best_node) std::fill(best_node + i0, best_node + i1, YK_NONE);
+        if (best_need) std::fill(best_need + i0, best_need + i1, 0u);
+    };
+    if (nlive == 0) { write_empty(0, n); return YK_OK; }   // no node: no victim is on a present node
+
+    const int D = e->D;
+    cudaStream_t s = e->stream;
+    CK(grow(e->pn_pos, e->maxN));
+    rc = filter_order(e);
+    if (rc) return rc;
+    yk_pn_pos_kernel<<<(nlive + 255) / 256, 256, 0, s>>>(e->f_val_out.p, (int)nlive, e->pn_pos.p);
+    CK(cudaGetLastError());
+    e->st.other_launches += 1;
+    const auto bits = [](uint32_t x) { return x ? 32 - __builtin_clz(x) : 0; };
+    const int pbits = std::max(1, bits(nlive - 1));
+    const size_t row_words = 2 * (size_t)k + 3;
+    const uint32_t rows_cap = (uint32_t)std::min<size_t>(PN_ROWS, std::max<size_t>(1, PN_WORDS / row_words));
+    for (uint32_t c0 = 0; c0 < n;) {
+        // a chunk is whole lists: it ends before the list that would take it past PN_ENTRIES entries or rows_cap lists (a
+        // longer list is a chunk of its own)
+        uint32_t c1 = c0 + 1;
+        while (c1 < n && c1 - c0 < rows_cap && victim_off[c1 + 1] - victim_off[c0] <= PN_ENTRIES) ++c1;
+        const uint32_t rows = c1 - c0, raw = victim_off[c1] - victim_off[c0];
+        const size_t head_words = 2 * (size_t)rows + 1;
+        CK(grow(e->h_pn_in, head_words + 2 * (size_t)raw));
+        uint32_t* h_asks = e->h_pn_in.p;
+        uint32_t* h_off = h_asks + rows;
+        uint32_t* h_vic = h_off + rows + 1;
+        uint32_t* h_node = h_vic + raw;
+        uint32_t m = 0;   // entries kept: victims bound to a present node, of asks that are present
+        for (uint32_t r = 0; r < rows; ++r) {
+            const uint32_t i = c0 + r;
+            h_asks[r] = asks[i];
+            h_off[r] = m;
+            if (e->a_state[asks[i]] == yk::ST_ABSENT) continue;
+            for (uint32_t j = victim_off[i]; j < victim_off[i + 1]; ++j) {
+                const uint32_t v = victims[j], node = e->a_bound[v];
+                if (node >= e->maxN || !e->n_present[node]) continue;
+                h_vic[m] = v; h_node[m] = node; ++m;
+            }
+        }
+        h_off[rows] = m;
+        if (m) {
+            const int end_bit = pbits + std::max(1, bits(rows - 1));
+            CK(grow(e->pn_in, head_words + 2 * (size_t)raw));
+            CK(grow(e->pn_key_in, m)); CK(grow(e->pn_key_out, m)); CK(grow(e->pn_val_in, m)); CK(grow(e->pn_val_out, m));
+            CK(grow(e->pn_head, m)); CK(grow(e->pn_incl, m)); CK(grow(e->pn_gask, m)); CK(grow(e->pn_gnode, m));
+            CK(grow(e->pn_goff, (size_t)m + 1)); CK(grow(e->pn_start, m)); CK(grow(e->pn_res, m)); CK(grow(e->pn_vreq, (size_t)D * m));
+            CK(grow(e->pn_out, rows * row_words)); CK(grow(e->h_pn_out, rows * row_words));
+            size_t sort_b = 0, scan_b = 0;
+            CK(cub::DeviceRadixSort::SortPairs(nullptr, sort_b, e->pn_key_in.p, e->pn_key_out.p, e->pn_val_in.p, e->pn_val_out.p,
+                                               (int)m, 0, end_bit, s));
+            CK(cub::DeviceScan::InclusiveSum(nullptr, scan_b, e->pn_head.p, e->pn_incl.p, (int)m, s));
+            CK(grow(e->pn_cub, std::max(sort_b, scan_b)));
+            uint32_t* d_asks = e->pn_in.p;
+            uint32_t* d_off = d_asks + rows;
+            uint32_t* d_vic = d_off + rows + 1;
+            uint32_t* d_node = d_vic + raw;
+            CK(cudaMemcpyAsync(d_asks, h_asks, 4 * (head_words + m), cudaMemcpyHostToDevice, s));
+            CK(cudaMemcpyAsync(d_node, h_node, 4 * (size_t)m, cudaMemcpyHostToDevice, s));
+            const unsigned blocks = (m + 255) / 256;
+            yk_pn_key_kernel<<<blocks, 256, 0, s>>>(d_off, (int)rows, d_node, e->pn_pos.p, (int)m, pbits, e->pn_key_in.p,
+                                                    e->pn_val_in.p);
+            size_t tb = sort_b;   // stable: the entries of one (list, node) group stay in list order
+            CK(cub::DeviceRadixSort::SortPairs(e->pn_cub.p, tb, e->pn_key_in.p, e->pn_key_out.p, e->pn_val_in.p, e->pn_val_out.p,
+                                               (int)m, 0, end_bit, s));
+            yk_pn_head_kernel<<<blocks, 256, 0, s>>>(e->pn_key_out.p, (int)m, e->pn_head.p);
+            tb = scan_b;
+            CK(cub::DeviceScan::InclusiveSum(e->pn_cub.p, tb, e->pn_head.p, e->pn_incl.p, (int)m, s));
+            yk_pn_group_kernel<<<blocks, 256, 0, s>>>(D, e->pn_key_out.p, e->pn_val_out.p, e->pn_incl.p, (int)m, pbits, d_asks, d_vic,
+                                                      e->f_val_out.p, e->d_areq.p, e->maxA, e->pn_gask.p, e->pn_gnode.p,
+                                                      e->pn_goff.p, e->pn_vreq.p);
+            CK(cudaMemsetAsync(e->pn_start.p, 0, 4 * (size_t)m, s));
+            // every (list, node) group is one query of the single-query search, start 0: the answers are yk_preemption_search's
+            yk_preempt_kernel<<<(m + 3) / 4, 128, 0, s>>>(
+                D, e->d_total.p, e->d_avail.p, e->maxN, e->d_taint.p, e->d_label.p, e->d_flags.p, e->d_areq.p, e->d_atol.p,
+                e->d_aneed.p, e->d_adeny.p, e->d_anode.p, e->maxA, (int)m, e->pn_gask.p, e->pn_gnode.p, e->pn_goff.p, e->pn_vreq.p,
+                m, e->pn_start.p, e->pn_res.p);
+            yk_pn_rank_kernel<<<(rows + 3) / 4, 128, 0, s>>>(d_off, e->pn_incl.p, e->pn_res.p, e->pn_gnode.p, (int)rows, skip, k,
+                                                             e->pn_out.p);
+            CK(cudaGetLastError());
+            CK(cudaMemcpyAsync(e->h_pn_out.p, e->pn_out.p, 4 * rows * row_words, cudaMemcpyDeviceToHost, s));
+            // 5 kernels of yk_preempt_nodes.cuh / yk_kernels.cuh, the cub radix sort (histogram, exclusive sum, one onesweep
+            // pass per 8 key bits) and the cub scan (init, scan)
+            e->st.other_launches += 5 + 2 + (end_bit + 7) / 8 + 2;
+            e->st.h2d_bytes += 4 * (head_words + 2 * (size_t)m);
+            e->st.d2h_bytes += 4 * rows * row_words;
+        }
+        CK(cudaStreamSynchronize(s));
+        if (e->h_f_flag[0]) return e->fail(YK_ERR_RANGE, "yk_preemption_nodes: NaN node score (zero total on a weighted resource)");
+        if (!m) { write_empty(c0, c1); c0 = c1; continue; }
+        for (uint32_t r = 0; r < rows; ++r) {
+            const uint32_t i = c0 + r;
+            const uint32_t* o = e->h_pn_out.p + r * row_words;
+            if (k) memcpy(nodes_out + (size_t)i * k, o, 4 * (size_t)k);
+            if (k && need_out) memcpy(need_out + (size_t)i * k, o + k, 4 * (size_t)k);
+            if (n_fit) n_fit[i] = o[2 * (size_t)k];
+            if (best_node) best_node[i] = o[2 * (size_t)k + 1];
+            if (best_need) best_need[i] = o[2 * (size_t)k + 2];
+        }
+        c0 = c1;
     }
     return YK_OK;
 }

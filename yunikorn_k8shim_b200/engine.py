@@ -23,7 +23,7 @@ EXPORTS = [
     "yk_abi_version", "yk_create", "yk_destroy", "yk_nodes_upsert", "yk_nodes_remove", "yk_queues_set", "yk_queues_priority",
     "yk_apps_upsert", "yk_apps_remove", "yk_apps_user", "yk_user_limits_set", "yk_asks_upsert", "yk_asks_remove", "yk_release", "yk_cycle",
     "yk_ask_states", "yk_nodes_available", "yk_evaluate", "yk_evaluate_reserve", "yk_node_scores", "yk_filter_nodes",
-    "yk_preemption_search", "yk_set_exchange",
+    "yk_preemption_search", "yk_preemption_nodes", "yk_set_exchange",
     "yk_peer_export", "yk_peer_import", "yk_peer_enable", "yk_stats",
     "yk_stats_reset", "yk_strerror", "yk_last_error",
 ]
@@ -318,6 +318,26 @@ class Engine:
         out = np.zeros(len(ask), dtype=np.int32)
         self._ck(self._lib.yk_preemption_search(self._h, C.c_uint32(len(ask)), _p(ask), _p(node), _p(off), _p(flat), _p(start), _p(out)))
         return out
+
+    def preemption_nodes(self, asks, victim_lists, k=0, skip=0):
+        """victim_lists: per ask the allocated asks that may be preempted for it, in victim order -> (nodes[n][k], need[n][k],
+        n_fit[n], best_node[n], best_need[n]) uint32: per ask, the fitting nodes of fit rank skip .. skip+k-1 in the cycle's node
+        order with the victims each needs (YK_NONE / 0 past the end), how many nodes fit, and the one needing the fewest"""
+        asks = _arr(asks, np.uint32)
+        n = asks.size
+        if len(victim_lists) != n:
+            raise ValueError(f"expected {n} victim lists, got {len(victim_lists)}")
+        off = np.zeros(n + 1, dtype=np.uint32)
+        off[1:] = np.cumsum([len(v) for v in victim_lists])
+        victims = np.concatenate([np.asarray(v, dtype=np.uint32).ravel() for v in victim_lists]) if n else np.zeros(0, np.uint32)
+        victims = _arr(victims, np.uint32)
+        nodes = np.zeros((n, k), dtype=np.uint32)
+        need = np.zeros((n, k), dtype=np.uint32)
+        n_fit, best_node, best_need = (np.zeros(n, dtype=np.uint32) for _ in range(3))
+        self._ck(self._lib.yk_preemption_nodes(self._h, C.c_uint32(n), _p(asks), _p(off), _p(victims) if victims.size else None,
+                                               C.c_uint32(skip), C.c_uint32(k), _p(nodes) if k else None, _p(need) if k else None,
+                                               _p(n_fit), _p(best_node), _p(best_need)))
+        return nodes, need, n_fit, best_node, best_need
 
     def set_exchange(self, fn):
         cb = ALLGATHER_FN(fn) if fn is not None else C.cast(None, ALLGATHER_FN)

@@ -76,6 +76,9 @@ def run(s, max_bindings=-1):
     total = [[int(x) for x in row] for row in s.node_total]
     avail = [[int(x) for x in row] for row in s.node_avail]
     ids = [i.encode() for i in s.node_id]
+    for n in range(N):   # a +Inf and a -Inf share: the score is NaN, rejected up front like the C++ oracle and the library
+        if math.isnan(node_score(s.policy, w, total[n], avail[n])):
+            raise ValueError(f"node {n} scores NaN")
     req = [[int(x) for x in row] for row in s.ask_req]
     Q = s.n_queues
     children = [[] for _ in range(Q)]

@@ -114,6 +114,13 @@ typedef enum {
 #define YK_FLAG_DEVICE_COMMIT 4u    /* commit on the device whenever the cycle is eligible, also where the order is not made of
                                       uniform runs (yk_lattice_kernel: exact, no bitmap read-back, no host work per ask, but
                                       measured slower than the host commit there) */
+#define YK_FLAG_BINPACKING_DEVICE 8u /* also take eligible cycles under the binpacking node sort, in auto and device commit: every
+                                      maximal uniform run is decided by one ordered capacity fill on the device (a node's key never
+                                      rises under binpacking, so the front node fills to its capacity before the next one: one sort,
+                                      one 64-bit scan, one search per ask, csrc/yk_uniform.h); gangs that may need a roll-back and
+                                      stretches cut inside a gang go to the host commit.  auto prices a fill at its measured cost
+                                      against the host commit's per-ask cost (DESIGN.md §6.4).  Unset: binpacking cycles always take
+                                      the sweep + host commit path.  Same bindings either way. */
 
 typedef struct yk_engine yk_engine;
 

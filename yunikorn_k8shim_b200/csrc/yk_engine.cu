@@ -50,6 +50,9 @@ constexpr int NODE_TILE = YK_SWEEP_THREADS * NPT;
 constexpr int RD_MIN = 10000;               // fewest pending asks for which a mask-free cycle starts on the device commit
 constexpr double RD_US_PER_ASK = 0.19;      // whole cycle per ask on the round commit (config 2: 8.7-10.1 ms / 50 000)
 constexpr double RD_HOST_US_PER_ASK = 0.28; // ... and on the sweep + host commit (config 2: 12.4-19.7 ms / 50 000)
+// binpacking fill (yk_uniform.h, YK_FLAG_BINPACKING_DEVICE), measured on H100 by scripts/binpack_prof.py (DESIGN.md §6.4)
+constexpr double BP_FILL_US = 140.0;        // whole cycle per fill (runny config 2: 737 ms / 5 198 fills), whatever the run's length
+constexpr double BP_HOST_US_PER_ASK = 0.1;  // whole cycle per ask on the sweep + host commit (0.106-0.137 us on the three shapes)
 
 inline size_t round_up(size_t v, size_t m) { return (v + m - 1) / m * m; }
 
@@ -266,6 +269,7 @@ struct yk_engine {
     bool lt_allowed = true;                  // !YK_FLAG_HOST_COMMIT, single GPU
     int lt_force = 0;                        // YK_FLAG_DEVICE_COMMIT / YK_COMMIT=device: every eligible cycle commits on the device
     bool lt_auto = false;                    // the default: eligible cycles whose order is made of long uniform runs commit on the device
+    bool bp_device = false;                  // YK_FLAG_BINPACKING_DEVICE: binpacking cycles are eligible too (one fill per run)
     bool lt_active = false;                  // this cycle runs (so far) on the device commit
     bool cycle_has_gang = false;             // some pending ask of this cycle is a gang member
     bool order_enqueued = false;             // device_order() of this cycle is already on the stream
@@ -535,7 +539,9 @@ int un_ensure(yk_engine* e) {
     size_t t0 = 0, t1 = 0;
     CK(cub::DeviceRadixSort::SortPairs(nullptr, t0, e->d_un_ekey[0].p, e->d_un_ekey[1].p, e->d_un_enode[0].p, e->d_un_enode[1].p, (int)ykun::UN_EMAX, 0, 64, e->stream));
     CK(cub::DeviceRadixSort::SortPairs(nullptr, t1, e->d_un_rkey[0].p, e->d_un_rkey[1].p, e->d_un_rrn[0].p, e->d_un_rrn[1].p, (int)std::max<size_t>(N, 1), 0, 64, e->stream));
-    e->un_cub_bytes = std::max(t0, t1);
+    size_t t2 = 0;   // the binpacking fill's scan
+    CK(cub::DeviceScan::InclusiveSum(nullptr, t2, e->d_un_rkey[0].p, e->d_un_rkey[1].p, (int)std::max<size_t>(N, 1), e->stream));
+    e->un_cub_bytes = std::max(std::max(t0, t1), t2);
     CK(e->d_un_cub.alloc(e->un_cub_bytes));
     e->un_alloc = true;
     return YK_OK;
@@ -565,6 +571,35 @@ cudaError_t un_attempt(yk_engine* e, const ykun::Args& a) {
     }
 }
 
+// One binpacking fill (yk_uniform.h): the run's keys at L = 1, sorted; capacities per sorted position, scanned; decide,
+// select, apply.  Once the keys are sorted, ekey holds the capacities and bk their inclusive sum.
+template <int D>
+cudaError_t un_fill_d(yk_engine* e, const ykun::Args& a) {
+    cudaStream_t s = e->stream;
+    const int nb = (a.nlive + 255) / 256;
+    ykun::un_reset_kernel<<<1, 1, 0, s>>>(a.g);
+    ykun::un_depth_kernel<D><<<nb, 256, 0, s>>>(a);   // a.L == 1
+    size_t tb = e->un_cub_bytes;
+    cudaError_t rc = cub::DeviceRadixSort::SortPairs(e->d_un_cub.p, tb, a.ekey, const_cast<unsigned long long*>(a.skey), a.enode,
+                                                     const_cast<uint32_t*>(a.snode), a.nlive, 0, 64, s);
+    if (rc != cudaSuccess) return rc;
+    ykun::un_fill_cap_kernel<D><<<nb, 256, 0, s>>>(a);
+    tb = e->un_cub_bytes;
+    rc = cub::DeviceScan::InclusiveSum(e->d_un_cub.p, tb, a.ekey, a.bk, a.nlive, s);
+    if (rc != cudaSuccess) return rc;
+    ykun::un_fill_decide_kernel<<<1, 1, 0, s>>>(a);
+    ykun::un_fill_select_kernel<<<(a.R + 255) / 256, 256, 0, s>>>(a);
+    ykun::un_apply_rekey_kernel<D><<<nb, 256, 0, s>>>(a);
+    return cudaGetLastError();
+}
+cudaError_t un_fill(yk_engine* e, const ykun::Args& a) {
+    switch (e->D) {
+        case 1: return un_fill_d<1>(e, a); case 2: return un_fill_d<2>(e, a); case 3: return un_fill_d<3>(e, a);
+        case 4: return un_fill_d<4>(e, a); case 5: return un_fill_d<5>(e, a); case 6: return un_fill_d<6>(e, a);
+        case 7: return un_fill_d<7>(e, a); default: return un_fill_d<8>(e, a);
+    }
+}
+
 // The node order after uniform runs: only the windowed kernel reads it, so it is rebuilt (stable sort of the re-keyed entries,
 // which un_apply_rekey_kernel left in rank order) when a windowed stretch follows, not after every run.
 int un_reorder(yk_engine* e) {
@@ -584,7 +619,7 @@ int un_reorder(yk_engine* e) {
 }
 
 // One uniform run: entries [off, off + R) of the staged batch (h_lt_asks; results land in d_lt_res at the same offset),
-// through ykun::uniform_run with un_attempt as the attempt.
+// through ykun::uniform_run with un_attempt as the attempt (un_fill under binpacking).
 int lt_uniform(yk_engine* e, size_t off, size_t R, bool has_gang, int* status, size_t* consumed) {
     const int nlive = (int)e->nlive;
     int rc = un_ensure(e);
@@ -602,10 +637,11 @@ int lt_uniform(yk_engine* e, size_t off, size_t R, bool has_gang, int* status, s
     a.bk = e->d_un_bk.p; a.cnt = e->d_un_cnt.p;
     a.rkey = e->d_un_rkey[0].p; a.okey = e->d_un_rkey[1].p; a.rrn = e->d_un_rrn[0].p; a.orn = e->d_un_rrn[1].p;
     a.res = e->d_lt_res.p + off; a.g = e->d_un_g.p;
+    const bool bp = e->cfg.policy == YK_POLICY_BINPACKING;
     auto attempt = [&](int L, ykun::Globals& g) -> int {
         a.L = L;
         CK(cudaEventRecord(e->ev_l0, s));
-        CK(un_attempt(e, a));
+        CK(bp ? un_fill(e, a) : un_attempt(e, a));
         CK(cudaEventRecord(e->ev_l1, s));
         CK(cudaMemcpyAsync(e->h_un_g.p, e->d_un_g.p, sizeof(ykun::Globals), cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
@@ -613,13 +649,15 @@ int lt_uniform(yk_engine* e, size_t off, size_t R, bool has_gang, int* status, s
         cudaEventElapsedTime(&ms, e->ev_l0, e->ev_l1);
         e->st.lattice_ms += ms;
         e->st.lattice_launches += 1;
-        e->st.other_launches += 16;   // 6 kernels of yk_uniform.cuh + one cub radix sort (histogram, exclusive sum, 8 onesweep passes)
+        // 6 kernels of yk_uniform.cuh + one cub radix sort (histogram, exclusive sum, 8 onesweep passes); a fill: 6 kernels, the
+        // sort, a cub scan (init, scan)
+        e->st.other_launches += bp ? 18 : 16;
         e->st.d2h_bytes += sizeof(ykun::Globals);
         g = e->h_un_g[0];
         return YK_OK;
     };
     rc = ykun::uniform_run(e->D, e->w.w, a.req, e->n_total.p, e->maxN, e->by_rank.p, nlive, (int)R, e->un_depth, e->st, attempt,
-                           status, consumed);
+                           status, consumed, bp);
     if (*status == ykun::U_DONE || *status == ykun::U_STOPPED) e->un_ord_stale = true;
     return rc;
 }
@@ -737,7 +775,8 @@ int lt_batch(yk_engine* e, size_t B, int* status, size_t* done, std::vector<uint
         return lt_rounds(e, off, len, st, consumed);
     };
     auto stretch = yklt::route_stretches(!e->lt_force, e->cm.t, e->ord.insensitive, e->rd_taints, e->h_lt_asks.p, rounds, window);
-    const int rc = yklt::run_segments(e->un_segs, e->h_lt_meta.p, uniform, stretch, status, done);
+    const int rc = e->cfg.policy == YK_POLICY_BINPACKING ? yklt::run_segments(e->un_segs, e->h_lt_meta.p, uniform, yklt::hand_off, status, done)
+                                                         : yklt::run_segments(e->un_segs, e->h_lt_meta.p, uniform, stretch, status, done);
     if (rc) return rc;
     if (*done) {
         CK(cudaMemcpyAsync(e->h_lt_res.p, e->d_lt_res.p, 4 * *done, cudaMemcpyDeviceToHost, s));
@@ -1199,6 +1238,7 @@ int yk_create(const yk_config* cfg, yk_engine** out) {
     e->lt_allowed = !(cfg->flags & YK_FLAG_HOST_COMMIT) && cfg->world <= 1;
     e->lt_auto = true;
     if (cfg->flags & YK_FLAG_DEVICE_COMMIT) e->lt_force = 1;
+    e->bp_device = (cfg->flags & YK_FLAG_BINPACKING_DEVICE) != 0;
     if (const char* cm = getenv("YK_COMMIT")) {
         if (!strcmp(cm, "host")) e->lt_allowed = false;
         if (!strcmp(cm, "device")) e->lt_force = 1;
@@ -1551,7 +1591,8 @@ int run_lattice(yk_engine* e, Cycle& c, bool& handoff) {
     if (rc) return rc;
     Slot& A = e->slot[0];
     yklt::Loop lp{e->ord, e->cm.t, e->lt_shape_ids, e->a_sigid.data(), A.asks, A.snap, c.result,
-                  e->h_lt_meta.p, e->h_lt_shp.p, e->h_lt_sig.p, e->un_segs, e->lt_plan_ready, e->un_min, e->nlive == 0,
+                  e->h_lt_meta.p, e->h_lt_shp.p, e->h_lt_sig.p, e->un_segs, e->lt_plan_ready,
+                  e->cfg.policy == YK_POLICY_BINPACKING ? 1 : e->un_min, e->nlive == 0,
                   e->ord.insensitive ? (size_t)e->maxA : (size_t)e->batch, c.max_bindings, c.n, e->st};
     if (e->nlive && !A.asks.empty()) {   // the initial order's NaN flag (device_order) is checked before the first batch
                                           // commits anything: a failed cycle must leave the node tables as they were
@@ -1665,9 +1706,12 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
     double begin_ms = 0;
     bool gang_too_big = false;
     setup_commit_tables(e);
-    // device commit: forced (every eligible cycle), or automatic (cycles whose asks come in long uniform runs: yk_uniform.h)
-    const bool force_lattice = e->lt_allowed && e->lt_force && e->cfg.policy == YK_POLICY_FAIR;
-    const bool auto_lattice = e->lt_allowed && !e->lt_force && e->lt_auto && e->un_min > 0 && e->cfg.policy == YK_POLICY_FAIR;
+    // device commit: forced (every eligible cycle), or automatic (cycles whose asks come in long uniform runs: yk_uniform.h);
+    // binpacking cycles only under YK_FLAG_BINPACKING_DEVICE, and never on the round commit
+    const bool bp = e->cfg.policy == YK_POLICY_BINPACKING;
+    const bool dev_policy = e->cfg.policy == YK_POLICY_FAIR || (bp && e->bp_device);
+    const bool force_lattice = e->lt_allowed && e->lt_force && dev_policy;
+    const bool auto_lattice = e->lt_allowed && !e->lt_force && e->lt_auto && e->un_min > 0 && dev_policy;
     e->worker.submit([&] {
         const double t_b = now_ms();
         pending.clear();
@@ -1679,7 +1723,7 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
         // (and whether every pending ask is free of masks -- yklt::round_eligible -- for the round commit)
         uint64_t taints = 0;
         if (auto_lattice) for (uint32_t n = 0; n < e->n_hi; ++n) if (e->n_present[n]) taints |= e->n_taint[n];
-        bool maskfree = auto_lattice;
+        bool maskfree = auto_lattice && !bp;
         for (uint32_t a = 0; a < e->a_hi; ++a) {
             uint8_t& st = e->a_state[a];
             if (st == yk::ST_ABSENT || st == yk::ST_ALLOCATED) continue;
@@ -1766,7 +1810,7 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
     bool lattice = false;
     size_t bsz0 = e->batch;
     if (force_lattice) {
-        const yklt::Eligibility el = yklt::eligible(e->cm.t, e->n_hi, e->n_present.data(), e->n_total.p, e->maxN, e->n_rank.data(), pending, &e->ranks_unique, &e->cycle_has_gang);
+        const yklt::Eligibility el = yklt::eligible(e->cm.t, e->n_hi, e->n_present.data(), e->n_total.p, e->maxN, e->n_rank.data(), pending, &e->ranks_unique, &e->cycle_has_gang, e->bp_device);
         lattice = el.ok;
         if (lattice && ins) bsz0 = e->maxA;   // the whole static order in one launch
     }
@@ -1789,7 +1833,7 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
             run = 1;
         }
         if (longest >= (size_t)e->un_min || round_screen) {
-            const yklt::Eligibility el = yklt::eligible(e->cm.t, e->n_hi, e->n_present.data(), e->n_total.p, e->maxN, e->n_rank.data(), pending, &e->ranks_unique, &e->cycle_has_gang);
+            const yklt::Eligibility el = yklt::eligible(e->cm.t, e->n_hi, e->n_present.data(), e->n_total.p, e->maxN, e->n_rank.data(), pending, &e->ranks_unique, &e->cycle_has_gang, e->bp_device);
             if (el.ok) {
                 // signature ids double as shape numbers: equal signatures request equal vectors; two signatures with one request
                 // only make the (rare, here) windowed stretches see one more shape
@@ -1802,13 +1846,18 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
                 if (!rc) {
                     const size_t B0 = e->slot[0].asks.size();
                     yklt::build_meta(e->cm.t, e->lt_shape_ids, e->a_sigid.data(), e->slot[0].asks, e->h_lt_meta.p, e->h_lt_shp.p, e->h_lt_sig.p);
-                    ykun::plan_segments(e->h_lt_meta.p, e->h_lt_shp.p, e->h_lt_sig.p, (int)B0, e->un_min, e->un_segs);
+                    ykun::plan_segments(e->h_lt_meta.p, e->h_lt_shp.p, e->h_lt_sig.p, (int)B0, bp ? 1 : e->un_min, e->un_segs);
                     // measured costs (H100, bench.py device_commit / host_commit arms): a uniform run ~0.2-0.3 ms whatever its
                     // length (16 launches, one round trip), a windowed ask ~0.35 us, an ask on the host commit ~0.08-0.13 us
                     // (the host side gets a 30 % margin); a round stretch is priced in whole-cycle time per ask on both sides
                     // (scripts/round_prof.py), which is how it was measured
                     double dev_us = 0, host_us = 0;
-                    for (const ykun::Segment& sg : e->un_segs) {
+                    // binpacking: a fill per run at its fixed cost; a stretch hands the rest of the cycle to the host commit
+                    if (bp) for (const ykun::Segment& sg : e->un_segs) {
+                        dev_us += sg.uniform ? BP_FILL_US : BP_HOST_US_PER_ASK * sg.len;
+                        host_us += BP_HOST_US_PER_ASK * sg.len;
+                    }
+                    else for (const ykun::Segment& sg : e->un_segs) {
                         const bool rounds = !sg.uniform && yklt::round_eligible(e->cm.t, ins, e->rd_taints, e->slot[0].asks.data() + sg.off, (size_t)sg.len);
                         dev_us += sg.uniform ? 250.0 : (rounds ? RD_US_PER_ASK : 0.35) * sg.len;
                         host_us += (rounds ? RD_HOST_US_PER_ASK : 0.7 * 0.08) * sg.len;

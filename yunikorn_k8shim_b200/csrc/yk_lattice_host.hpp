@@ -78,12 +78,25 @@ constexpr size_t UN_EMAX = (size_t)4 << 20;   // generated elements per attempt 
 // The attempts of one uniform run of R asks requesting `req`, on the live nodes `live` (totals column-major, leading
 // dimension ldn).  attempt(L, g) runs one attempt at depth L and leaves its Globals in g; a non-zero return is an error and
 // is passed on.  Afterwards *status is U_DONE / U_STOPPED with *consumed entries decided, U_FALLBACK (nothing was applied:
-// the windowed commit takes the run) or U_NAN (a node scores NaN after the commit).
+// the windowed commit takes the run) or U_NAN (a node scores NaN after the commit).  Under binpacking an attempt is one
+// ordered capacity fill (yk_uniform.h), made once: attempt(1, g).
 template <class Attempt>
 inline int uniform_run(int D, const double* w, const int64_t* req, const int64_t* n_total, size_t ldn, const uint32_t* live, int nlive,
-                       int R, int first_override, yk_stats_t& st, Attempt&& attempt, int* status, size_t* consumed) {
+                       int R, int first_override, yk_stats_t& st, Attempt&& attempt, int* status, size_t* consumed,
+                       bool binpacking = false) {
     *status = U_FALLBACK; *consumed = 0;
     if (nlive == 0 || R == 0) return 0;
+    if (binpacking) {
+        if ((size_t)nlive > UN_EMAX) return 0;   // the keys do not fit the element buffers: fallback
+        Globals g{};
+        const int rc = attempt(1, g);
+        if (rc) return rc;
+        if (g.status == U_FALLBACK) return 0;
+        if (g.status == U_NAN || g.nan) { *status = U_NAN; return 0; }
+        *status = g.status; *consumed = (size_t)g.consumed;
+        st.uniform_runs++; st.uniform_asks += (uint64_t)g.consumed; st.uniform_elements += (uint64_t)nlive;
+        return 0;
+    }
     int L = first_depth(R, nlive);
     // no node takes the request more often than its TOTAL allows: beyond that depth nothing is ever cut
     int64_t capmax = 0;
@@ -213,7 +226,8 @@ inline size_t estimate_windows(const uint32_t* shp, const uint32_t* sig, size_t 
 }
 
 // What the lattice commit relies on (DESIGN.md "lattice commit"):
-//   fair node sort; weights >= 0 and weighted totals >= 0 (a node's key must not decrease when it is allocated to);
+//   fair node sort; weights >= 0 and weighted totals >= 0 (a node's key must not decrease when it is allocated to; under
+//   binpacking, which a caller may allow for the binpacking fill, it must not increase);
 //   NodeID ranks unique (element order is (key, rank, j)); every gang's members request the same vector (a gang never
 //   straddles two runs, so a failed gang is undone inside one sub-run).
 struct Eligibility {
@@ -222,12 +236,13 @@ struct Eligibility {
 };
 
 // ranks_unique: when the caller already knows whether the live nodes' ranks are distinct (the engine checks it where it sorts
-// the nodes by rank), else nullptr; any_gang: when it already knows whether any pending ask is a gang member.
+// the nodes by rank), else nullptr; any_gang: when it already knows whether any pending ask is a gang member; binpacking_ok:
+// the binpacking node sort is accepted (YK_FLAG_BINPACKING_DEVICE).
 inline Eligibility eligible(const yk::CommitTables& t, uint32_t n_hi, const uint8_t* n_present, const int64_t* n_total,
                             size_t ldn, const uint32_t* n_rank, const std::vector<uint32_t>& pending, const bool* ranks_unique = nullptr,
-                            const bool* any_gang = nullptr) {
+                            const bool* any_gang = nullptr, bool binpacking_ok = false) {
     Eligibility e;
-    if (t.policy != 0u) { e.why = "binpacking node sort"; return e; }
+    if (t.policy != 0u && !(t.policy == 1u && binpacking_ok)) { e.why = "binpacking node sort"; return e; }
     for (int k = 0; k < t.D; ++k) if (t.w[k] < 0.0 || t.w[k] != t.w[k]) { e.why = "negative node-sort weight"; return e; }
     for (int k = 0; k < t.D; ++k) {
         if (t.w[k] == 0.0) continue;
@@ -286,6 +301,15 @@ inline int run_segments(const std::vector<ykun::Segment>& segs, const uint32_t* 
         *status = st;
         if (st != ST_DONE || cons < (size_t)sg.len) break;
     }
+    return 0;
+}
+
+// The window callback of run_segments under binpacking, where a batch is planned with min_run = 1 (every segment a maximal
+// uniform run, each decided by one fill): a segment the fill cannot decide -- a run whose gang may need a roll-back
+// (U_FALLBACK), or a stretch cut inside a gang whose members carry different signatures -- and everything after it goes to
+// the host commit.
+inline int hand_off(size_t, size_t, int* status, size_t* consumed) {
+    *status = ST_HANDOFF; *consumed = 0;
     return 0;
 }
 

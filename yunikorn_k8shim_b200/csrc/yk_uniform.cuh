@@ -58,6 +58,20 @@ __global__ void __launch_bounds__(256) un_apply_rekey_kernel(const Args a) {
     if (rekey_item<D>(a, i)) a.g->nan = 2;   // a NaN score AFTER the commit (status stays: the host reports it)
 }
 
+// the binpacking fill (yk_uniform.h): un_depth_kernel at L = 1, a radix sort, then these three around a cub inclusive scan
+template <int D>
+__global__ void __launch_bounds__(256) un_fill_cap_kernel(const Args a) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p < a.nlive) fill_cap_item<D>(a, p);
+}
+
+__global__ void un_fill_decide_kernel(const Args a) { fill_decide(a); }
+
+__global__ void __launch_bounds__(256) un_fill_select_kernel(const Args a) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q < a.R) fill_select_item(a, q, a.g->valid);
+}
+
 __global__ void un_order_kernel(const Args a) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= a.nlive) return;

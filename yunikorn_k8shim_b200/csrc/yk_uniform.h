@@ -51,9 +51,11 @@ struct Args {
     int L;                           // elements generated per node
     int R;                           // asks in the run
     int insensitive, has_gang;
-    unsigned long long* ekey; uint32_t* enode;         // [nlive * L] generated, (rank, j) order
+    unsigned long long* ekey; uint32_t* enode;         // [nlive * L] generated, (rank, j) order (binpacking fill, once sorted:
+                                                       // the capacity per sorted position)
     const unsigned long long* skey; const uint32_t* snode;   // the same, stably sorted by key
-    unsigned long long* bk;          // [nlive] key of element (n, L) where the node was cut, else KEY_INF
+    unsigned long long* bk;          // [nlive] key of element (n, L) where the node was cut, else KEY_INF (binpacking fill, once
+                                     // sorted: the inclusive sum of the capacities)
     uint32_t* cnt;                   // [node index] elements taken per node; zero outside an attempt
     unsigned long long* rkey; unsigned long long* rrn;           // [nlive] re-keyed order entries in rank order
     const unsigned long long* okey; const unsigned long long* orn;   // ... sorted by key
@@ -198,6 +200,56 @@ LT_FN int rekey_item(const Args& a, int i) {
     a.rkey[i] = key;
     a.rrn[i] = ((uint64_t)r[2 * D + 2] >> 32 << 32) | (uint64_t)n;
     return key == KEY_INF ? 1 : 0;
+}
+
+// ---- binpacking: one ordered capacity fill per run (DESIGN.md §6.4) ----------------------------------------------------
+// Under `binpacking` (key = 1 - usage) a node's key never INCREASES when it is allocated to.  So the node at the front of the
+// ascending (key, rank) order among those that accept the run and have room keeps taking its asks until its capacity for the
+// request is gone; a node before it refused the run by its masks or flags or had no room, and neither changes during the
+// run.  Ask q of the run therefore goes to the node where the inclusive prefix sum of the capacities, in that order, first
+// exceeds q: element_item at L = 1 gives the keys (KEY_INF where the node takes nothing), a stable radix sort of them in
+// rank order gives skey / snode, then fill_cap_item (into ekey), a 64-bit inclusive scan of ekey into bk (nodes x R
+// overflows 32 bits), fill_decide, fill_select_item and the unchanged apply / re-key.  No depth, no retry, no chain.
+
+// sorted position p: how many asks of the run its node takes (at most R; 0 past the nodes that take any)
+template <int D>
+LT_FN void fill_cap_item(const Args& a, int p) {
+    if (a.skey[p] == KEY_INF) { a.ekey[p] = 0; return; }
+    const int64_t* r = a.rec + (size_t)a.snode[p] * a.RS;
+    a.ekey[p] = (unsigned long long)cap_of<D>(true, r, r + D, a.req, (int64_t)a.R);   // a finite key: usable, accepts, cap >= 1
+}
+
+// what the fill amounts to (one thread, after the scan): decide() without RETRY; g.valid = the asks that get a node
+LT_FN void fill_decide(const Args& a) {
+    Globals& g = *a.g;
+    const unsigned long long total = a.nlive > 0 ? a.bk[a.nlive - 1] : 0ull;
+    const unsigned m = total < (unsigned long long)a.R ? (unsigned)total : (unsigned)a.R;
+    g.valid = m;
+    if (g.nan) { g.status = U_NAN; g.consumed = 0; return; }
+    if (m < (unsigned)a.R) {   // asks m, m+1, ... find nothing
+        if (a.has_gang) { g.status = U_FALLBACK; g.consumed = 0; return; }   // a gang may have to be rolled back: the host commit does that
+        if (a.insensitive) { g.status = U_DONE; g.consumed = a.R; return; }
+        g.status = U_STOPPED; g.consumed = (int)m + 1;
+        return;
+    }
+    g.status = U_DONE; g.consumed = a.R;
+}
+
+// ask q of the run (select_item's contract): the node of the first sorted position whose inclusive sum exceeds q
+LT_FN void fill_select_item(const Args& a, int q, unsigned m) {
+    if ((unsigned)q >= m) { a.res[q] = NONE; return; }
+    int lo = 0, hi = a.nlive - 1;   // bk[nlive - 1] >= m > q
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (a.bk[mid] > (unsigned long long)q) hi = mid; else lo = mid + 1;
+    }
+    const uint32_t n = a.snode[lo];
+    a.res[q] = n;
+#if defined(__CUDA_ARCH__)
+    atomicAdd(&a.cnt[n], 1u);
+#else
+    a.cnt[n] += 1u;
+#endif
 }
 
 // ---- host side: where the uniform runs of a batch are ------------------------------------------------------------

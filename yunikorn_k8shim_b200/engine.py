@@ -39,6 +39,7 @@ class Config(C.Structure):
 FLAG_NO_ROW_SHARING = 1
 FLAG_HOST_COMMIT = 2
 FLAG_DEVICE_COMMIT = 4
+FLAG_BINPACKING_DEVICE = 8
 
 
 class Stats(C.Structure):
@@ -125,10 +126,12 @@ class Engine:
     """One yk_engine.  Method names and arguments mirror include/ykgpu.h one to one.
 
     commit: where the ordered commit runs -- "auto" (the library's default: on the device for cycles made of long uniform runs,
-    sweep + host commit otherwise), "host" (YK_FLAG_HOST_COMMIT), "device" (YK_FLAG_DEVICE_COMMIT: every eligible cycle)."""
+    sweep + host commit otherwise), "host" (YK_FLAG_HOST_COMMIT), "device" (YK_FLAG_DEVICE_COMMIT: every eligible cycle).
+    binpacking_device: under the binpacking node sort, let "auto" and "device" commit eligible cycles on the device too, one
+    ordered capacity fill per uniform run (YK_FLAG_BINPACKING_DEVICE); off, binpacking cycles stay on the host commit."""
 
     def __init__(self, D=4, policy=0, weights=None, max_nodes=1024, max_asks=4096, max_apps=64, max_queues=8,
-                 batch=0, device=-1, rank=0, world=1, share_rows=True, commit="auto"):
+                 batch=0, device=-1, rank=0, world=1, share_rows=True, commit="auto", binpacking_device=False):
         self._lib = load_library()
         cfg = Config()
         cfg.abi_version = self._lib.yk_abi_version()
@@ -145,6 +148,8 @@ class Engine:
         cfg.max_nodes, cfg.max_asks, cfg.max_apps, cfg.max_queues = max_nodes, max_asks, max_apps, max_queues
         cfg.device, cfg.rank, cfg.world = device, rank, world
         cfg.flags = (0 if share_rows else FLAG_NO_ROW_SHARING) | {"auto": 0, "host": FLAG_HOST_COMMIT, "device": FLAG_DEVICE_COMMIT}[commit]
+        if binpacking_device:
+            cfg.flags |= FLAG_BINPACKING_DEVICE
         self.D = D
         self._h = C.c_void_p()
         rc = self._lib.yk_create(C.byref(cfg), C.byref(self._h))

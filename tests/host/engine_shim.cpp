@@ -6,6 +6,7 @@
 // `-m gpu` tests.
 #include "../../yunikorn_k8shim_b200/csrc/yk_commit.hpp"
 #include "../../yunikorn_k8shim_b200/csrc/yk_orderer.hpp"
+#include "shim_tables.hpp"
 
 #include <algorithm>
 #include <cstdint>
@@ -70,19 +71,6 @@ void sweep_row_avx512(const SoAView& v, const int64_t* rq, uint64_t tol, uint64_
 }  // namespace
 
 
-// queue priority properties for the next run (priority.offset / priority.policy = fence); NULL = defaults.  Test
-// harness convenience: keeps the long argument lists of the run functions unchanged.
-static const int32_t* g_q_prio_offset = nullptr;
-static const uint8_t* g_q_prio_fence = nullptr;
-extern "C" void host_set_queue_priority(const int32_t* offset, const uint8_t* fence) { g_q_prio_offset = offset; g_q_prio_fence = fence; }
-// user / group limits for the next run (same convenience): application users, then the entries [D][n] column-major
-static const uint32_t* g_p_user = nullptr; static uint32_t g_n_ul = 0;
-static const uint32_t* g_ul_queue = nullptr; static const uint32_t* g_ul_user = nullptr;
-static const int64_t* g_ul_max = nullptr; static int64_t* g_ul_alloc = nullptr;
-extern "C" void host_set_user_limits(const uint32_t* p_user, uint32_t n, const uint32_t* queue, const uint32_t* user, const int64_t* max, int64_t* alloc) {
-    g_p_user = p_user; g_n_ul = n; g_ul_queue = queue; g_ul_user = user; g_ul_max = max; g_ul_alloc = alloc;
-}
-
 namespace {
 struct Slot { std::vector<uint32_t> asks, reps, row_of; yk::Orderer::Snap snap; std::vector<uint32_t> fit; };
 }
@@ -103,22 +91,9 @@ static int engine_host_run_impl(
     uint32_t* out_ask, uint32_t* out_node, uint32_t* n_out, uint8_t* state_out, int64_t* avail_out /*[D][nN]*/, uint64_t* rows_out) {
     // ---- orderer ----
     yk::Orderer o;
-    std::vector<uint8_t> state(nA, yk::ST_PENDING), present(nP, 1);
-    std::vector<int64_t> p_alloc((size_t)D * nP, 0);
-    o.t.D = D; o.t.maxA = nA; o.t.maxP = nP; o.t.nq = nQ;
-    o.t.a_req = a_req; o.t.a_prio = a_prio; o.t.a_create = a_create; o.t.a_app = a_app; o.t.a_flags = a_flags; o.t.a_gang = a_gang;
-    // the per-ask cause table the engine keeps at upsert time (yk::Tables::a_cause): same rule, so the tests walk that branch
-    std::vector<uint8_t> a_cause(nA, 0);
-    for (uint32_t a = 0; a < nA; ++a) {
-        bool pos = false, neg = false;
-        for (int k = 0; k < D; ++k) { const int64_t v = a_req[(size_t)k * nA + a]; neg = neg || v < 0; pos = pos || v > 0; }
-        a_cause[a] = (a_flags[a] & 1u) ? yk::ST_SLOWPATH : ((neg || !pos) ? yk::ST_INVALID : 0);
-    }
-    o.t.a_cause = a_cause.data();
-    o.t.a_state = state.data(); o.t.p_queue = p_queue; o.t.p_submit = p_submit; o.t.p_present = present.data();
-    o.t.q_parent = q_parent; o.t.q_guar = q_guar; o.t.q_max = q_max; o.t.q_alloc = q_alloc; o.t.p_alloc = p_alloc.data(); o.t.q_sort = q_sort;
-    o.t.q_prio_offset = g_q_prio_offset; o.t.q_prio_fence = g_q_prio_fence;
-    o.t.p_user = g_p_user; o.t.n_ul = g_n_ul; o.t.ul_queue = g_ul_queue; o.t.ul_user = g_ul_user; o.t.ul_max = g_ul_max; o.t.ul_alloc = g_ul_alloc;
+    ShimTables tb;
+    wire_orderer(o.t, tb, D, nA, nP, nQ, a_req, a_prio, a_create, a_app, a_flags, a_gang, p_queue, p_submit, q_parent, q_guar, q_max,
+                 q_alloc, q_sort);
     std::vector<uint32_t> pending(nA);
     for (uint32_t i = 0; i < nA; ++i) pending[i] = i;
     o.begin_cycle(pending);
@@ -317,7 +292,7 @@ static int engine_host_run_impl(
         for (int k = 0; k < 4; ++k) rows_out[1 + k] = cm.dbg[k];
         for (int k = 0; k < 6; ++k) rows_out[5 + k] = cm.prof[k];
     }
-    for (uint32_t i = 0; i < nA; ++i) state_out[i] = state[i];
+    for (uint32_t i = 0; i < nA; ++i) state_out[i] = tb.state[i];
     for (uint32_t nn = 0; nn < nN; ++nn)
         for (int k = 0; k < D; ++k) avail_out[(size_t)k * nN + nn] = cm.node(nn).avail()[k];
     return 0;

@@ -1,6 +1,6 @@
 """Binpacking on the device commit (YK_FLAG_BINPACKING_DEVICE) on the GPU, through the C ABI: one ordered capacity fill per
 uniform run (csrc/yk_uniform.cuh).  Bindings, node choices, final availability and ask states must equal the oracle's; the
-fill counters must equal the CPU shim's (tests/host/binpack_shim.cpp) on the same snapshot; without the flag nothing
+fill counters must equal the CPU shim's (tests/host/device_shim.cpp) on the same snapshot; without the flag nothing
 changes."""
 import copy
 
@@ -8,8 +8,9 @@ import numpy as np
 import pytest
 
 from yunikorn_k8shim_b200 import synth
-from test_binpack_host import (BP, bp, bshim, config_shapes, infinite_shares, mid_node, mixed_signature_gangs,  # noqa: F401
-                               overcommitted, run as shim_run, shuffled_ranks)   # (bshim: the shim fixture)
+from device_shim import dshim  # noqa: F401  (dshim: the shim fixture)
+from test_binpack_host import (BP, bp, config_shapes, infinite_shares, mid_node, mixed_signature_gangs, overcommitted,
+                               run as shim_run, shuffled_ranks)
 from test_gpu_dims import ST_PENDING, YK_ERR_RANGE, nan_node, nan_repaired, widen
 import test_sessions as ts
 
@@ -159,7 +160,7 @@ def test_nan_score_is_a_clean_error(oracle, commit):
         assert e.stats()["lattice_cycles"] == 2
 
 
-def test_counters_equal_the_shim(oracle, bshim):
+def test_counters_equal_the_shim(oracle, dshim):
     """uniform runs, fills (lattice launches: one per fill, no other kernel runs), uniform asks and hand-offs.  The batch
     holds every ask: in a placement-insensitive order the engine decides the whole order in one batch, the shim in
     `batch`-sized ones"""
@@ -172,7 +173,7 @@ def test_counters_equal_the_shim(oracle, bshim):
         want = oracle.run(s)
         dev = _fill(s, want, batch=batch)
         c = []
-        rc, ask, node, _, _ = shim_run(bshim, s, stats=c, batch=batch)
+        rc, ask, node, _, _ = shim_run(dshim, s, stats=c, batch=batch)
         assert rc == 0 and np.array_equal(ask, want["ask"]) and np.array_equal(node, want["node"])
         c = c[0]
         assert (dev["uniform_runs"], dev["uniform_asks"], dev["lattice_handoffs"], dev["lattice_launches"]) == \

@@ -3,24 +3,19 @@
 speculative next batch, rewind, epochs with lazy order merges -- with the device sweep replaced by a plain CPU loop.
 Bindings, ask states and node availability must equal the oracle's, for every batch size / epoch length."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 from yunikorn_k8shim_b200 import synth
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 NONE = 0xFFFFFFFF
 
 
 @pytest.fixture(scope="module")
-def shim(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("engine") / "engine_shim.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-w", "-o", out,
-                           os.path.join(HERE, "host", "engine_shim.cpp")])
-    return C.CDLL(out)
+def shim():
+    from device_shim import load   # (device_shim imports this module)
+    return load("engine_shim")
 
 
 def _p(a):
@@ -73,7 +68,7 @@ def run_engine_host(shim, s, batch=256, epoch_limit=None, speculate=1, max_bindi
     n = C.c_uint32(0)
     state = np.zeros(max(A, 1), dtype=np.uint8)
     avail = np.zeros((D, max(N, 1)), dtype=np.int64)
-    nrows = np.zeros(16, dtype=np.uint64)   # engine shim: [0] rows swept; lattice shim: its counters
+    nrows = np.zeros(32, dtype=np.uint64)   # engine shim: [0] rows swept; device shim: its counters
     rc = getattr(shim, fn)(
         C.c_int(D), C.c_uint32(s.policy), _p(k["w"]),
         C.c_uint32(N), _p(k["total"]), _p(k["avail"]), _p(k["taint"]), _p(k["label"]), _p(k["nflags"]), _p(k["rank"]),

@@ -1,33 +1,23 @@
 """Semantics tightened in round 2, checked on the oracle, the independent Python restatement, the host engine shim (real
-orderer + real host commit) and the lattice shim (real orderer + the device commit's code compiled for the CPU):
+orderer + real host commit) and the device shim (real orderer + the device commit's code compiled for the CPU):
   * a weighted resource with total == 0: Go's float division gives +-Inf shares (0/0 = NaN is skipped), not "absent";
   * gangs are all-or-nothing whichever member is the bad one (ADVICE round 1: the first-reached member used to be dropped
     alone, the rest scheduled as a smaller gang);
   * slow-path members of a sunk gang are reported whether or not the order is placement-sensitive."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 from yunikorn_k8shim_b200 import synth
 from oracle import py_oracle
+import device_shim
 from test_engine_host import run_engine_host
-
-HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 @pytest.fixture(scope="module")
-def shims(tmp_path_factory):
-    d = tmp_path_factory.mktemp("r2")
-    out = {}
-    for name in ("engine_shim", "lattice_shim"):
-        so = str(d / f"{name}.so")
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-w", "-o", so,
-                               os.path.join(HERE, "host", f"{name}.cpp")])
-        out[name] = C.CDLL(so)
-    return out
+def shims():
+    return {"engine_shim": device_shim.load("engine_shim"), "device_shim": device_shim.load("device_shim")}
 
 
 def everywhere(shims, oracle, s, batch=64):
@@ -36,8 +26,8 @@ def everywhere(shims, oracle, s, batch=64):
     assert list(want["ask"]) == p["ask"] and list(want["node"]) == p["node"] and list(want["state"]) == p["state"]
     rc, ask, node, state, avail = run_engine_host(shims["engine_shim"], s, batch=batch)
     assert rc == 0 and np.array_equal(ask, want["ask"]) and np.array_equal(node, want["node"]) and np.array_equal(state, want["state"])
-    rc, ask, node, state, avail = run_engine_host(shims["lattice_shim"], s, batch=batch, fn="lattice_host_run")
-    if rc != 100:
+    rc, ask, node, state, avail = device_shim.run(shims["device_shim"], s, rounds=0, batch=batch)
+    if rc != device_shim.INELIGIBLE:
         assert rc == 0 and np.array_equal(ask, want["ask"]) and np.array_equal(node, want["node"]) and np.array_equal(state, want["state"])
     return want
 

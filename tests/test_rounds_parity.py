@@ -4,7 +4,7 @@ tests/test_rounds_host.py runs the header's `#else` branches.  On the device the
 and a cross-warp exclusive minimum (block_prefmin), a warp-bounded merge (merge_into), a register bitonic sort
 (block_sort_fast), block_scan, warp_append and the red_* reductions.  A round that stops too early is still exact -- the
 next round or a single step decides the same ask, only more slowly -- so bindings alone can hide a device fault.  The shim
-(tests/host/rounds_shim.cpp) runs the same deterministic rounds under the engine's own driver, so here every case runs
+(tests/host/device_shim.cpp) runs the same deterministic rounds under the engine's own driver, so here every case runs
 twice: through the C ABI under the default `auto` commit, and through the shim with the same window, guard and uniform
 minimum.  Bindings, node choices, final availability and ask states must equal the oracle's; passes, single steps, round
 asks, hand-offs and uniform asks must equal the shim's exactly.
@@ -20,8 +20,8 @@ import pytest
 
 from yunikorn_k8shim_b200 import synth
 from oracle import py_oracle
-from test_rounds_host import ALL, check, infinite_shares, maskfree, rshim, shrunk  # noqa: F401  (rshim: the shim fixture)
-from test_engine_host import run_engine_host
+from device_shim import check, dshim, run  # noqa: F401  (dshim: the shim fixture)
+from test_rounds_host import ALL, infinite_shares, maskfree, shrunk
 from test_gpu_dims import ST_PENDING, YK_ERR_RANGE, _device_eligible, extreme, nan_node, nan_repaired, widen
 import test_sessions as ts
 
@@ -30,7 +30,7 @@ NO_UNIFORM = 1 << 30      # YK_UNIFORM_MIN that no run reaches: identical asks s
                           # device commit off)
 GUARD = 32                # the engine's own guard (ykrd::GUARD)
 WCAP = 1024               # candidates per round at most (ykrd::WCAP)
-# device counter -> shim counter (tests/host/rounds_shim.cpp stats order, test_rounds_host.STATS)
+# device counter -> shim counter (device_shim.STATS)
 COUNTERS = {"round_passes": "passes", "round_single_steps": "singles", "round_asks": "round_asks",
             "lattice_handoffs": "handoffs", "uniform_asks": "uniform_asks"}
 PY_ORACLE_PAIRS = 1_500_000   # node x ask pairs above which the Python oracle takes minutes (it is an exhaustive argmin)
@@ -228,10 +228,12 @@ def all_runs():
             yield name, r
 
 
-def _shim(rshim, oracle, r):
+def _shim(dshim, oracle, r):
     """the shim on the run's snapshot and knobs -> (oracle result or None for a NaN snapshot, counters by device name)"""
-    want, st = check(rshim, oracle, r.snap, tag=repr(r), uniform=(r.umin, 0), window=r.window, guard=r.guard,
+    want, st = check(dshim, oracle, r.snap, tag=repr(r), uniform=(r.umin, 0), window=r.window, guard=r.guard,
                      batch=1 << 16, max_bindings=r.mb)
+    if want is None:
+        return None, None
     c = {dev: st[sh] for dev, sh in COUNTERS.items()}
     c.update(parked=st["parked"], stretches=st["round_stretches"])
     return want, c
@@ -264,10 +266,10 @@ def _device(monkeypatch, r, want):
 # ---- A. on the GPU ----
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", list(CASES))
-def test_round_commit_matches_oracle_and_shim(rshim, oracle, monkeypatch, name):
+def test_round_commit_matches_oracle_and_shim(dshim, oracle, monkeypatch, name):
     ran = 0
     for r in case_runs(name):
-        want, shim = _shim(rshim, oracle, r)
+        want, shim = _shim(dshim, oracle, r)
         if want is None:
             continue                              # a NaN score: test_nan_snapshot_on_the_round_route
         st = _device(monkeypatch, r, want)
@@ -284,7 +286,7 @@ def test_round_commit_matches_oracle_and_shim(rshim, oracle, monkeypatch, name):
 
 
 @pytest.mark.gpu
-def test_nan_snapshot_on_the_round_route(rshim, oracle, monkeypatch):
+def test_nan_snapshot_on_the_round_route(dshim, oracle, monkeypatch):
     """node 5 scores NaN: the cycle on the round route is a clean YK_ERR_RANGE (nothing bound, every ask pending, the node
     tables unchanged); with node 5 repaired the next cycle on the same engine is the oracle's, by rounds, with the shim's
     counters"""
@@ -292,7 +294,7 @@ def test_nan_snapshot_on_the_round_route(rshim, oracle, monkeypatch):
     s = nan_node()
     t = nan_repaired(s)
     r = Run(t)
-    want, shim = _shim(rshim, oracle, r)
+    want, shim = _shim(dshim, oracle, r)
     assert shim["round_asks"] == t.n_asks
     A, N = np.arange(s.n_asks), np.arange(s.n_nodes)
     _knobs(monkeypatch, r)
@@ -358,12 +360,12 @@ def test_fixtures_are_round_eligible():
 
 
 @pytest.mark.parametrize("name", list(CASES))
-def test_shim_matches_oracle(rshim, oracle, name):
+def test_shim_matches_oracle(dshim, oracle, name):
     """the shim (the kernel's own code, CPU build) decides every fixture as the oracle does and hits what the case targets;
     the GPU test compares the device's counters with these"""
     ran = 0
     for r in case_runs(name):
-        want, c = _shim(rshim, oracle, r)
+        want, c = _shim(dshim, oracle, r)
         if want is None:
             continue
         assert (c["round_asks"] > 0) == r.rounds, (r, c)
@@ -373,12 +375,12 @@ def test_shim_matches_oracle(rshim, oracle, name):
     assert ran >= (8 if name.startswith("dims") else 1)
 
 
-def test_nan_snapshot_fixture(rshim, oracle):
+def test_nan_snapshot_fixture(dshim, oracle):
     with pytest.raises(RuntimeError):
         oracle.run(nan_node())
-    rc, *_ = run_engine_host(rshim, nan_node(), fn="rounds_host_run", batch=1 << 16)
+    rc, *_ = run(dshim, nan_node(), batch=1 << 16)
     assert rc == YK_ERR_RANGE
-    _, c = _shim(rshim, oracle, Run(nan_repaired(nan_node())))
+    _, c = _shim(dshim, oracle, Run(nan_repaired(nan_node())))
     assert c["round_asks"] == 5000
 
 

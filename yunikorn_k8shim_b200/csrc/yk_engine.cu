@@ -774,9 +774,8 @@ int lt_batch(yk_engine* e, size_t B, int* status, size_t* done, std::vector<uint
         }
         return lt_rounds(e, off, len, st, consumed);
     };
-    auto stretch = yklt::route_stretches(!e->lt_force, e->cm.t, e->ord.insensitive, e->rd_taints, e->h_lt_asks.p, rounds, window);
-    const int rc = e->cfg.policy == YK_POLICY_BINPACKING ? yklt::run_segments(e->un_segs, e->h_lt_meta.p, uniform, yklt::hand_off, status, done)
-                                                         : yklt::run_segments(e->un_segs, e->h_lt_meta.p, uniform, stretch, status, done);
+    const int rc = yklt::route_batch(e->cfg.policy == YK_POLICY_BINPACKING, !e->lt_force, e->cm.t, e->ord.insensitive, e->rd_taints,
+                                     e->h_lt_asks.p, e->un_segs, e->h_lt_meta.p, uniform, rounds, window, status, done);
     if (rc) return rc;
     if (*done) {
         CK(cudaMemcpyAsync(e->h_lt_res.p, e->d_lt_res.p, 4 * *done, cudaMemcpyDeviceToHost, s));
@@ -1244,7 +1243,7 @@ int yk_create(const yk_config* cfg, yk_engine** out) {
         if (!strcmp(cm, "device")) e->lt_force = 1;
         if (!strcmp(cm, "auto")) { e->lt_auto = true; e->lt_force = 0; e->lt_allowed = !(cfg->flags & YK_FLAG_HOST_COMMIT) && cfg->world <= 1; }
     }
-    e->lt_RS = (2 * D + 3 + 3) / 4 * 4;
+    e->lt_RS = yklt::record_words(D);
     T(e->d_rec.alloc(N * (size_t)e->lt_RS)); T(e->d_ord[0].alloc(N)); T(e->d_ord[1].alloc(N)); T(e->d_rank.alloc(N));
     T(e->d_lt_cur.alloc(1)); T(e->d_lt_hdr.alloc(yklt::H_WORDS)); T(e->d_lt_ub.alloc(8));
     T(e->d_lt_asks.alloc(A)); T(e->d_lt_meta.alloc(A)); T(e->d_lt_shp.alloc(A)); T(e->d_lt_sig.alloc(A)); T(e->d_lt_res.alloc(A));
@@ -1436,19 +1435,6 @@ int yk_apps_remove(yk_engine* e, uint32_t n, const uint32_t* idx) {
     return YK_OK;
 }
 
-// what keeps an ask out of the passes whatever the cluster looks like (yk::Tables::a_cause): the slow-path flag, or a request
-// that is not strictly greater than zero ([EXT] preAllocateCheck)
-static uint8_t ask_cause(const yk_engine* e, uint32_t x) {
-    if (e->a_flags[x] & 1u) return yk::ST_SLOWPATH;
-    bool pos = false;
-    for (int k = 0; k < e->D; ++k) {
-        const int64_t v = e->a_req[(size_t)k * e->maxA + x];
-        if (v < 0) return yk::ST_INVALID;
-        if (v > 0) pos = true;
-    }
-    return pos ? 0 : yk::ST_INVALID;
-}
-
 int yk_asks_upsert(yk_engine* e, uint32_t a, const uint32_t* idx, const int64_t* req, const uint64_t* tol,
                    const uint64_t* need, const uint64_t* deny, const int32_t* prio, const int64_t* create_seq,
                    const uint32_t* app, const uint32_t* required_node, const uint32_t* flags, const uint32_t* gang) {
@@ -1483,7 +1469,7 @@ int yk_asks_upsert(yk_engine* e, uint32_t a, const uint32_t* idx, const int64_t*
         if (full) e->sigs.reset(e->maxA);
         else for (uint32_t i = 0; i < a; ++i) e->sigs.retire(x0 + i);
         for (uint32_t i = 0; i < a; ++i) e->a_sig[x0 + i] = yk::ask_signature(sv, x0 + i);
-        for (uint32_t i = 0; i < a; ++i) e->a_cause[x0 + i] = ask_cause(e, x0 + i);
+        for (uint32_t i = 0; i < a; ++i) e->a_cause[x0 + i] = yk::ask_cause(e->D, e->a_req.p, e->maxA, e->a_flags.data(), x0 + i);
         e->a_hi = std::max(e->a_hi, x0 + a);
         if (!full && e->sigs.n > 2 * e->maxA) {   // too many stale numbers: renumber every present ask
             e->sigs.reset(e->maxA);
@@ -1512,7 +1498,7 @@ int yk_asks_upsert(yk_engine* e, uint32_t a, const uint32_t* idx, const int64_t*
         e->a_create[x] = create_seq[i];
         e->a_app[x] = app[i];
         e->a_flags[x] = flags ? flags[i] : 0;
-        e->a_cause[x] = ask_cause(e, x);
+        e->a_cause[x] = yk::ask_cause(e->D, e->a_req.p, e->maxA, e->a_flags.data(), x);
         e->a_gang[x] = gang ? gang[i] : YK_NONE;
         e->a_state[x] = yk::ST_PENDING;
         e->a_bound[x] = YK_NONE;
@@ -1592,7 +1578,7 @@ int run_lattice(yk_engine* e, Cycle& c, bool& handoff) {
     Slot& A = e->slot[0];
     yklt::Loop lp{e->ord, e->cm.t, e->lt_shape_ids, e->a_sigid.data(), A.asks, A.snap, c.result,
                   e->h_lt_meta.p, e->h_lt_shp.p, e->h_lt_sig.p, e->un_segs, e->lt_plan_ready,
-                  e->cfg.policy == YK_POLICY_BINPACKING ? 1 : e->un_min, e->nlive == 0,
+                  yklt::min_run(e->cfg.policy == YK_POLICY_BINPACKING, e->un_min), e->nlive == 0,
                   e->ord.insensitive ? (size_t)e->maxA : (size_t)e->batch, c.max_bindings, c.n, e->st};
     if (e->nlive && !A.asks.empty()) {   // the initial order's NaN flag (device_order) is checked before the first batch
                                           // commits anything: a failed cycle must leave the node tables as they were
@@ -1846,7 +1832,7 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
                 if (!rc) {
                     const size_t B0 = e->slot[0].asks.size();
                     yklt::build_meta(e->cm.t, e->lt_shape_ids, e->a_sigid.data(), e->slot[0].asks, e->h_lt_meta.p, e->h_lt_shp.p, e->h_lt_sig.p);
-                    ykun::plan_segments(e->h_lt_meta.p, e->h_lt_shp.p, e->h_lt_sig.p, (int)B0, bp ? 1 : e->un_min, e->un_segs);
+                    ykun::plan_segments(e->h_lt_meta.p, e->h_lt_shp.p, e->h_lt_sig.p, (int)B0, yklt::min_run(bp, e->un_min), e->un_segs);
                     // measured costs (H100, bench.py device_commit / host_commit arms): a uniform run ~0.2-0.3 ms whatever its
                     // length (16 launches, one round trip), a windowed ask ~0.35 us, an ask on the host commit ~0.08-0.13 us
                     // (the host side gets a 30 % margin); a round stretch is priced in whole-cycle time per ask on both sides

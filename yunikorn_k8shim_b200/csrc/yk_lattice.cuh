@@ -17,8 +17,7 @@ __global__ void __launch_bounds__(yklt::THREADS, 1) yk_lattice_kernel(const yklt
     yklt::lattice_batch<D>(a, s);
 }
 
-// node records + the cycle's initial order from what the key kernel and the stable radix sort produced:
-// rec[n] = {available[D], total[D], taint, label, rank << 32 | flags}; ord[p] = {key, rank << 32 | node}
+// node records + the cycle's initial order from what the key kernel and the stable radix sort produced (yklt::init_node)
 __global__ void yk_lt_init_kernel(int D, const int64_t* __restrict__ total, const int64_t* __restrict__ avail, size_t ldn,
                                   const uint64_t* __restrict__ taint, const uint64_t* __restrict__ label,
                                   const uint32_t* __restrict__ flags, const uint32_t* __restrict__ rank,
@@ -26,16 +25,7 @@ __global__ void yk_lt_init_kernel(int D, const int64_t* __restrict__ total, cons
                                   int64_t* __restrict__ rec, int RS, yklt::Ent* __restrict__ ord) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= nlive) return;
-    const uint32_t n = sorted_node[p];
-    int64_t* r = rec + (size_t)n * RS;
-    for (int k = 0; k < D; ++k) { r[k] = avail[(size_t)k * ldn + n]; r[D + k] = total[(size_t)k * ldn + n]; }
-    r[2 * D] = (int64_t)taint[n];
-    r[2 * D + 1] = (int64_t)label[n];
-    r[2 * D + 2] = (int64_t)(((uint64_t)rank[n] << 32) | (uint64_t)flags[n]);
-    yklt::Ent e;
-    e.key = sorted_key[p];
-    e.rn = ((uint64_t)rank[n] << 32) | (uint64_t)n;
-    ord[p] = e;
+    yklt::init_node(D, p, total, avail, ldn, taint, label, flags, rank, sorted_key, sorted_node, rec, RS, ord);
 }
 
 // available of every live node back into the column-major table (position order = any order: each node once)

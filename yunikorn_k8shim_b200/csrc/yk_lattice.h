@@ -1,6 +1,6 @@
 // yk_lattice.h -- the device-resident ordered commit ("lattice commit"), single source:
 //   * compiled by nvcc it is the body of yk_lattice_kernel (one persistent CTA of 1024 threads, sm_90a);
-//   * compiled by g++ (tests/host/lattice_shim.cpp) the SAME code runs as a sequential emulation, so the CPU test suite
+//   * compiled by g++ (tests/host/device_shim.cpp) the SAME code runs as a sequential emulation, so the CPU test suite
 //     fuzzes the algorithm against the oracle without a GPU (test infrastructure; the product only ever runs the kernel).
 //
 // What it replaces: the reference's one-allocation-per-pass loop [EXT yunikorn-core Application.tryNodes / tryNode, entered
@@ -95,10 +95,33 @@ struct Ent { uint64_t key; uint64_t rn; };   // one position of the node order: 
 
 LT_HD bool ent_less(uint64_t k0, uint64_t r0, uint64_t k1, uint64_t r1) { return k0 < k1 || (k0 == k1 && r0 < r1); }
 
+// A node record: [0,D) available, [D,2D) total, [2D] taint, [2D+1] label, [2D+2] rank << 32 | flags, padded to whole
+// 32-byte lines
+LT_HD constexpr int record_words(int D) { return (2 * D + 3 + 3) / 4 * 4; }
+
+// Position p of the cycle's initial order, as the key kernel and the stable radix sort left it (sorted_key, sorted_node),
+// and its node's record of RS = record_words(D) words (yk_lt_init_kernel, one position per thread; the node tables are
+// column-major with leading dimension ldn)
+LT_HD void init_node(int D, int p, const int64_t* __restrict__ total, const int64_t* __restrict__ avail, size_t ldn,
+                     const uint64_t* __restrict__ taint, const uint64_t* __restrict__ label, const uint32_t* __restrict__ flags,
+                     const uint32_t* __restrict__ rank, const uint64_t* __restrict__ sorted_key,
+                     const uint32_t* __restrict__ sorted_node, int64_t* __restrict__ rec, int RS, Ent* __restrict__ ord) {
+    const uint32_t n = sorted_node[p];
+    int64_t* r = rec + (size_t)n * RS;
+    for (int k = 0; k < D; ++k) { r[k] = avail[(size_t)k * ldn + n]; r[D + k] = total[(size_t)k * ldn + n]; }
+    r[2 * D] = (int64_t)taint[n];
+    r[2 * D + 1] = (int64_t)label[n];
+    r[2 * D + 2] = (int64_t)(((uint64_t)rank[n] << 32) | (uint64_t)flags[n]);
+    Ent e;
+    e.key = sorted_key[p];
+    e.rn = ((uint64_t)rank[n] << 32) | (uint64_t)n;
+    ord[p] = e;
+}
+
 struct Args {
     uint32_t policy;
     double w[8];
-    int64_t* rec; int RS;                  // node records: [0,D) available, [D,2D) total, [2D] taint, [2D+1] label, [2D+2] rank<<32|flags
+    int64_t* rec; int RS;                  // node records (record_words / init_node)
     Ent* ord[2]; int* cur;                 // the node order, ping-pong; *cur = which buffer is current
     int nlive;
     const int64_t* a_req; size_t lda;      // ask table (column-major, as in yk_kernels.cuh)
@@ -743,7 +766,7 @@ LT_FN void lattice_batch(const Args& a, Shared<D>& s) {
             LT_SYNC();
             {   // the records: consecutive threads read consecutive words of one record (a few coalesced requests per
                 // record instead of one request per word)
-                constexpr int RW = (2 * D + 3 + 3) / 4 * 4;   // = a.RS
+                constexpr int RW = record_words(D);   // = a.RS
                 LT_FOR(x, P * RW) {
                     const int p = x / RW, w = x % RW;
                     if (w > 2 * D + 2) continue;

@@ -1,7 +1,7 @@
 // yk_lattice_host.hpp -- host side of the device commit (yk_lattice.h, yk_uniform.h): the per-entry meta words the kernel
 // reads, the test that decides whether a cycle may use the device commit at all, and the driver around the kernels (the
 // batch loop, the segment loop, a uniform run's attempts; settle and fill_batch, which the host commit uses too).  No CUDA
-// in here: csrc/yk_engine.cu drives the kernels with it and tests/host/lattice_shim.cpp drives their per-item code with it.
+// in here: csrc/yk_engine.cu drives the kernels with it and tests/host/device_shim.cpp drives their per-item code with it.
 #pragma once
 #include <chrono>
 #include <cstdint>
@@ -334,6 +334,19 @@ inline auto route_stretches(bool rounds_on, const yk::CommitTables& t, bool inse
         if (rounds_on && round_eligible(t, insensitive, taints, asks + off, len)) return rounds(off, len, status, consumed);
         return window(off, len, status, consumed);
     };
+}
+
+// The shortest uniform run of a cycle on the device commit (0: none): under binpacking every maximal run is one fill.
+inline int min_run(bool binpacking, int un_min) { return binpacking ? 1 : un_min; }
+
+// One planned batch of a cycle on the device commit (run_segments over the asks `asks`): under binpacking the stretches
+// between the uniform runs go to the host commit (hand_off), otherwise through route_stretches.
+template <class Uniform, class Rounds, class Window>
+inline int route_batch(bool binpacking, bool rounds_on, const yk::CommitTables& t, bool insensitive, uint64_t taints, const uint32_t* asks,
+                       const std::vector<ykun::Segment>& segs, const uint32_t* meta, Uniform&& uniform, Rounds&& rounds,
+                       Window&& window, int* status, size_t* consumed) {
+    if (binpacking) return run_segments(segs, meta, uniform, hand_off, status, consumed);
+    return run_segments(segs, meta, uniform, route_stretches(rounds_on, t, insensitive, taints, asks, rounds, window), status, consumed);
 }
 
 // What the device commit's batch loop works on; the caller owns all of it.

@@ -60,6 +60,21 @@ struct Tables {   // views into the engine's host tables
     int64_t* ul_alloc = nullptr;              // [D][n_ul] persistent: what the user holds there (updated at finish())
 };
 
+inline bool strictly_gt_zero(const int64_t* v, int d) {
+    bool pos = false;
+    for (int k = 0; k < d; ++k) { if (v[k] < 0) return false; if (v[k] > 0) pos = true; }
+    return pos;
+}
+
+// What keeps ask a out of the passes whatever the cluster looks like (Tables::a_cause): the slow-path flag, or a request
+// (column-major, leading dimension lda) that is not strictly greater than zero ([EXT] preAllocateCheck)
+inline uint8_t ask_cause(int D, const int64_t* a_req, size_t lda, const uint32_t* a_flags, uint32_t a) {
+    if (a_flags[a] & 1u) return ST_SLOWPATH;
+    int64_t rq[8];
+    for (int k = 0; k < D; ++k) rq[k] = a_req[(size_t)k * lda + a];
+    return strictly_gt_zero(rq, D) ? 0 : ST_INVALID;
+}
+
 class Orderer {
 public:
     struct QState {
@@ -144,11 +159,6 @@ public:
     std::vector<std::pair<uint32_t, uint8_t>>* jr = nullptr;   // where set_state logs (the batch being filled)
 
     int D() const { return t.D; }
-    static bool strictly_gt_zero(const int64_t* v, int d) {
-        bool pos = false;
-        for (int k = 0; k < d; ++k) { if (v[k] < 0) return false; if (v[k] > 0) pos = true; }
-        return pos;
-    }
     int64_t req(uint32_t a, int k) const { return t.a_req[(size_t)k * t.maxA + a]; }
 
     void begin_cycle(const std::vector<uint32_t>& pending_asks) {
@@ -256,13 +266,7 @@ public:
     // not meet them again; confirm / fail_in_place / finish give them their final state), one bad member sinks the gang.
     void extend_static(size_t want) {
         const int d = t.D;
-        auto cause_of = [&](uint32_t a) -> uint8_t {
-            if (t.a_cause) return t.a_cause[a];
-            if (t.a_flags[a] & 1u) return ST_SLOWPATH;
-            int64_t rq[8];
-            for (int k2 = 0; k2 < d; ++k2) rq[k2] = req(a, k2);
-            return strictly_gt_zero(rq, d) ? 0 : ST_INVALID;
-        };
+        auto cause_of = [&](uint32_t a) -> uint8_t { return t.a_cause ? t.a_cause[a] : ask_cause(d, t.a_req, t.maxA, t.a_flags, a); };
         static_order.reserve(std::min<size_t>(static_order.size() + (want == (size_t)-1 ? (size_t)t.maxA : want), (size_t)t.maxA + 1));
         while (static_order.size() - static_next < want && sa_app < static_apps.size()) {
             const auto& v = ap_asks[static_apps[sa_app]];

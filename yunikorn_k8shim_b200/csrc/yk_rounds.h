@@ -1,6 +1,6 @@
 // yk_rounds.h -- the device-resident ordered commit for MASK-FREE stretches ("round commit"), single source like
 // yk_lattice.h: nvcc builds it into yk_rounds_kernel (one persistent CTA, yk_rounds.cuh), g++ into plain loops for the CPU
-// test suite (tests/host/rounds_shim.cpp).
+// test suite (tests/host/device_shim.cpp).
 //
 // What it replaces: the same one-allocation-per-pass loop as yk_lattice.h under the `fair` node sort, for a stretch of
 // consecutive asks in a placement-insensitive order that carry no masks (no required / forbidden labels, no node name, every

@@ -2,7 +2,7 @@
 // order that all request the same vector and carry the same predicate signature (the replicas of one deployment / the
 // executors of one job; the reference's own benchmark, pkg/shim/scheduler_perf_test.go:283-288, is one such run of 50 000).
 // Single source like yk_lattice.h: the per-item bodies below are called by the sm_90a kernels in yk_uniform.cuh and, as
-// plain loops, by tests/host/lattice_shim.cpp (test infrastructure).
+// plain loops, by tests/host/device_shim.cpp (test infrastructure).
 //
 // What it replaces: the same one-allocation-per-pass loop as yk_lattice.h [EXT yunikorn-core Application.tryNodes, entered
 // per pair through pkg/cache/scheduler_callback.go:196-198 -> pkg/cache/context.go:683-703], under the `fair` node sort.

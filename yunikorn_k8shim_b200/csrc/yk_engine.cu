@@ -48,7 +48,7 @@ constexpr int NODE_TILE = YK_SWEEP_THREADS * NPT;
 // round commit (yk_rounds.h), measured on H100 by scripts/round_prof.py (DESIGN.md §6.3): mask-free fair cycles of 10 000
 // asks and more are faster on it, 5 000 are not
 constexpr int RD_MIN = 10000;               // fewest pending asks for which a mask-free cycle starts on the device commit
-constexpr double RD_US_PER_ASK = 0.19;      // whole cycle per ask on the round commit (config 2: 8.7-10.1 ms / 50 000)
+constexpr double RD_US_PER_ASK = 0.16;      // whole cycle per ask on the round commit (config 2: 7.4-8.2 ms / 50 000)
 constexpr double RD_HOST_US_PER_ASK = 0.28; // ... and on the sweep + host commit (config 2: 12.4-19.7 ms / 50 000)
 // binpacking fill (yk_uniform.h, YK_FLAG_BINPACKING_DEVICE), measured on H100 by scripts/binpack_prof.py (DESIGN.md §6.4)
 constexpr double BP_FILL_US = 140.0;        // whole cycle per fill (runny config 2: 737 ms / 5 198 fills), whatever the run's length
@@ -302,6 +302,7 @@ struct yk_engine {
     bool rd_maskfree = false;                   // this cycle: every pending ask is round-eligible (no gang, no masks)
     size_t rd_smem = 0;
     Dev<yklt::Ent> d_rd_spent; Dev<int> d_rd_hdr; Pin<int> h_rd_hdr;
+    Dev<int64_t> d_rd_req;                      // [maxA][D]: a stretch's requests in stretch order (ykrd::Args::sreq)
     Dev<uint32_t> pre_q; Dev<int64_t> pre_v; Dev<int32_t> pre_o;   // yk_preemption_search staging, grown on demand
     // yk_filter_nodes: its own node order (so a cycle's sort buffers are never touched) and per-chunk buffers, grown on demand
     Dev<uint64_t> f_key_in, f_key_out; Dev<uint32_t> f_val_in, f_val_out; Dev<uint8_t> f_cub; size_t f_cub_bytes = 0;
@@ -719,7 +720,7 @@ int lt_rounds(yk_engine* e, size_t off, size_t B, int* status, size_t* consumed)
     a.rec = e->d_rec.p; a.RS = e->lt_RS; a.ord[0] = e->d_ord[0].p; a.ord[1] = e->d_ord[1].p; a.cur = e->d_lt_cur.p;
     a.nlive = (int)e->nlive; a.spent = e->d_rd_spent.p;
     a.a_req = e->d_areq.p; a.lda = e->maxA; a.a_tol = e->d_atol.p; a.a_need = e->d_aneed.p; a.a_deny = e->d_adeny.p; a.a_node = e->d_anode.p;
-    a.asks = e->d_lt_asks.p + off; a.B = (int)B; a.res = e->d_lt_res.p + off; a.hdr = e->d_rd_hdr.p;
+    a.asks = e->d_lt_asks.p + off; a.B = (int)B; a.sreq = e->d_rd_req.p; a.res = e->d_lt_res.p + off; a.hdr = e->d_rd_hdr.p;
     a.window = std::max(1, std::min(e->rd_window, ykrd::WCAP)); a.guard = e->rd_guard;
     a.prof = e->lt_prof ? e->d_lt_prof.p + 16 : nullptr;
     CK(cudaEventRecord(e->ev_l0, s));
@@ -1259,7 +1260,7 @@ int yk_create(const yk_config* cfg, yk_engine** out) {
     if (const char* rm = getenv("YK_ROUND_MIN")) e->rd_min = std::max(0, atoi(rm));         // 0: no cycle starts on the round commit
     if (const char* rw = getenv("YK_ROUND_WINDOW")) e->rd_window = std::max(1, std::min(atoi(rw), ykrd::WCAP));
     if (const char* rg = getenv("YK_ROUND_GUARD")) e->rd_guard = std::max(0, atoi(rg));
-    T(e->d_rd_spent.alloc(N)); T(e->d_rd_hdr.alloc(ykrd::R_WORDS)); T(e->h_rd_hdr.alloc(ykrd::R_WORDS));
+    T(e->d_rd_spent.alloc(N)); T(e->d_rd_req.alloc(A * (size_t)D)); T(e->d_rd_hdr.alloc(ykrd::R_WORDS)); T(e->h_rd_hdr.alloc(ykrd::R_WORDS));
     T(e->d_lt_prof.alloc(32));   // [0, 16) the lattice kernel's phases, [16, 32) the round kernel's
     if (ok) T(cudaMemset(e->d_lt_prof.p, 0, 32 * sizeof(long long)));
     if (ok) T(lattice_setup(D, &e->lt_smem));

@@ -25,8 +25,12 @@
 // A guard ends the stretch when rounds stay short (fewer than `guard` asks per pass on average after the first 16 passes):
 // what has been decided stands, and the rest of the cycle goes to the host commit.
 #pragma once
+#include <assert.h>
 #include <stdint.h>
 #include "yk_lattice.h"
+#if !LT_DEV
+#include <vector>
+#endif
 
 namespace ykrd {
 
@@ -56,6 +60,8 @@ struct Args {
     const int64_t* a_req; size_t lda;      // ask table (column-major)
     const uint64_t* a_tol; const uint64_t* a_need; const uint64_t* a_deny; const uint32_t* a_node;
     const uint32_t* asks; int B;           // the stretch
+    int64_t* sreq;                         // [B][D] scratch: the stretch's requests in stretch order, written at its start
+                                           // (host: one is allocated when it is null)
     uint32_t* res;                         // [B] node index or NONE
     int* hdr;                              // [R_WORDS]
     int window;                            // candidates per round, 1..WCAP
@@ -66,6 +72,7 @@ enum { RP_EDGES = 0, RP_CAND, RP_SCAN, RP_APPLY, RP_SORT, RP_MERGE, RP_SINGLE, R
 
 struct Shared {
     int m, n_new, n_sp, hit, nan, keep;
+    long long prof_t;
     int64_t minreq[8];
     u64 ck[WCAP], cr[WCAP];                // candidate j: the new entry of S[j] after ask i+j (KEY_INF: S[j] rejects it)
     u64 ek[WCAP], er[WCAP];                // S[j] itself: the first W entries of order + side list
@@ -82,7 +89,7 @@ static_assert(THREADS <= 1024 && WCAP <= THREADS, "one candidate per thread, at 
 LT_FN bool ent_lt(u64 k0, u64 r0, u64 k1, u64 r1) { return yklt::ent_less(k0, r0, k1, r1); }
 
 // exclusive prefix minimum of the pairs (k, r)[0, n), n <= THREADS, into (pk, pr); (KEY_INF, KEY_INF) is neutral
-LT_NI void block_prefmin(Shared& s, int n) {
+LT_FN void block_prefmin(Shared& s, int n) {
 #if LT_DEV
     const int i = threadIdx.x, lane = i & 31, wp = i >> 5;
     u64 a = i < n ? s.ck[i] : KEY_INF, b = i < n ? s.cr[i] : KEY_INF;
@@ -115,6 +122,57 @@ LT_NI void block_prefmin(Shared& s, int n) {
         s.pk[i] = ma; s.pr[i] = mb;
         if (ent_lt(s.ck[i], s.cr[i], ma, mb)) { ma = s.ck[i]; mb = s.cr[i]; }
     }
+#endif
+}
+
+// ascending sort of the round's n <= THREADS new entries (key, sec), result in key/sec; (bkey, bsec) a second buffer.
+// Device, over the next power of two pn >= n only (a round of config 2 keeps ~320 new entries: 16 of the 32 warps sort,
+// the others only meet the barriers): each warp sorts its 32 entries in registers (a shuffle network, no barrier), then
+// runs of w merge pairwise into runs of 2w through shared memory, one barrier per level -- an entry's place in the merged
+// run is its index in its own run plus the entries of the other run before it (a binary search; ties, which only the
+// padding has, go to the first run).  Host: the same function as the lattice kernel's.
+LT_FN void sort_new(u64* key, u64* sec, int n, u64* bkey, u64* bsec) {
+#if LT_DEV
+    int pn = 32;
+    while (pn < n) pn <<= 1;
+    const int i = threadIdx.x;
+    const bool act = i < pn;   // whole warps
+    u64 k0 = i < n ? key[i] : KEY_INF, s0 = i < n ? sec[i] : KEY_INF;
+    if (act)
+        for (int k = 2; k <= 32; k <<= 1)
+            for (int j = k >> 1; j > 0; j >>= 1) {
+                const u64 k1 = __shfl_xor_sync(0xFFFFFFFFu, k0, j), s1 = __shfl_xor_sync(0xFFFFFFFFu, s0, j);
+                const bool up = (i & k & 31) == 0, lower = (i & j) == 0;   // (every warp's run ascends)
+                const bool other_less = k1 < k0 || (k1 == k0 && s1 < s0);
+                if ((lower == up) == other_less) { k0 = k1; s0 = s1; }   // keep the smaller when (lower == up), else the larger
+            }
+    u64 *sk = key, *ss = sec, *dk = bkey, *ds = bsec;
+    if (act) { sk[i] = k0; ss[i] = s0; }   // (each thread reads and writes only its own index until the barrier)
+    __syncthreads();
+    for (int w = 32; w < pn; w <<= 1) {
+        if (act) {
+            const int base = i & ~(2 * w - 1);
+            const bool second = (i & w) != 0;
+            const u64* ok = sk + (second ? base : base + w);   // the other run
+            const u64* os = ss + (second ? base : base + w);
+            int lo = 0, hi = w;   // entries of the other run before this one (the first run wins ties)
+            while (lo < hi) {
+                const int mid = (lo + hi) >> 1;
+                const bool before = second ? !ent_lt(k0, s0, ok[mid], os[mid]) : ent_lt(ok[mid], os[mid], k0, s0);
+                if (before) lo = mid + 1; else hi = mid;
+            }
+            const int p = base + (i & (w - 1)) + lo;
+            dk[p] = k0; ds[p] = s0;
+        }
+        u64* t = sk; sk = dk; dk = t;
+        t = ss; ss = ds; ds = t;
+        __syncthreads();
+        if (act) { k0 = sk[i]; s0 = ss[i]; }   // (dk was last read before that barrier)
+    }
+    if (sk != key && i < n) { key[i] = k0; sec[i] = s0; }
+    __syncthreads();
+#else
+    yklt::block_sort_fast(key, sec, n, bkey, bsec);
 #endif
 }
 
@@ -180,13 +238,40 @@ LT_FN bool spent_of(const int64_t* r, const int64_t* minreq) {
     return false;
 }
 
-// can node n (record r) take ask `ask`?  The lattice kernel's test: usable, masks, node name, capacity on every dimension
+// the staged request of stretch position i
 template <int D>
-LT_FN bool accepts_ask(const Args& a, const int64_t* r, uint32_t n, uint32_t ask, int64_t* req) {
-    for (int k = 0; k < D; ++k) req[k] = a.a_req[(size_t)k * a.lda + ask];
+LT_FN void req_of(const Args& a, int i, int64_t* q) {
+    for (int k = 0; k < D; ++k) q[k] = a.sreq[(size_t)i * D + k];
+}
+
+// Can node n (record r) take request q of stretch position i?  The lattice kernel's test without the masks and the node
+// name: a stretch routed here has no required or forbidden labels and no node name, and tolerates every live taint
+// (yklt::round_eligible), so only the flags and the capacity decide.  The host checks that the masks would have agreed.
+template <int D>
+LT_FN bool takes(const Args& a, const int64_t* r, uint32_t n, int i, const int64_t* q) {
     const uint32_t fl = (uint32_t)(uint64_t)r[2 * D + 2];
-    return yklt::fits<D>((fl & 1u) && !(fl & 2u), r, r + D, req) &&
-           yklt::accepts((uint64_t)r[2 * D], (uint64_t)r[2 * D + 1], n, a.a_tol[ask], a.a_need[ask], a.a_deny[ask], a.a_node[ask]);
+    bool ok = (fl & 1u) && !(fl & 2u);
+    for (int k = 0; k < D; ++k) {
+        const int64_t t = r[D + k] < 0 ? 0 : r[D + k], v = r[k] < 0 ? 0 : r[k];
+        ok = ok && q[k] <= t && q[k] <= v;
+    }
+#if !LT_DEV
+    if (ok) {
+        const uint32_t ask = a.asks[i];
+        assert(yklt::accepts((uint64_t)r[2 * D], (uint64_t)r[2 * D + 1], n, a.a_tol[ask], a.a_need[ask], a.a_deny[ask], a.a_node[ask]));
+    }
+#endif
+    (void)a; (void)n; (void)i;
+    return ok;
+}
+
+// the key of node record r once it has taken request q: yk_node_score inlined on values in registers (yklt::key_of is
+// a call that puts its arrays in local memory), the same double operations in the same order, so the same bits
+template <int D>
+LT_FN u64 key_after(const Args& a, const int64_t* r, const int64_t* q) {
+    int64_t av[D], tt[D];
+    for (int k = 0; k < D; ++k) { av[k] = r[k] - q[k]; tt[k] = r[D + k]; }
+    return yk_key_bits(yk_node_score(D, a.policy, a.w, tt, av, 1));
 }
 
 // the side list goes back into the order: ord[buf][hd, hd + n) merged with it into ord[buf ^ 1][0, n + nl)
@@ -198,21 +283,32 @@ LT_FN void flush_side(const Args& a, Shared& s, int& buf, int& hd, int& n, int& 
 
 // ---- the stretch -------------------------------------------------------------------------------------------------
 template <int D>
-LT_FN void rounds_stretch(const Args& a, Shared& s) {
+LT_FN void stretch(const Args& a, Shared& s) {
     const int RS = a.RS, nlive = a.nlive, B = a.B;
     int buf = *a.cur;
     int t = 0, status = yklt::ST_DONE, passes = 0, singles = 0;
 #if LT_DEV
-    long long prof_t = clock64();
+    long long& prof_t = s.prof_t;   // thread 0's clock; in shared memory, not in a register held through every round
+    LT_ONE prof_t = clock64();
 #endif
 
-    // ---- the smallest request of the stretch per dimension (requests of an ask that reaches a commit are >= 0) ----
+    // ---- the stretch's requests staged in stretch order, and the smallest per dimension (requests of an ask that
+    // reaches a commit are >= 0) ----
     LT_ONE { for (int k = 0; k < 8; ++k) s.minreq[k] = INT64_MAX; s.n_sp = 0; s.keep = 0; s.nan = 0; }
     LT_SYNC();
-    for (int k = 0; k < D; ++k) {
-        u64 my = KEY_INF;
-        LT_FOR(i, B) { const int64_t v = a.a_req[(size_t)k * a.lda + a.asks[i]]; const u64 c = v < 0 ? 0ull : (u64)v; my = c < my ? c : my; }
-        yklt::red_min64(reinterpret_cast<u64*>(&s.minreq[k]), my);
+    {
+        u64 my[D];
+        for (int k = 0; k < D; ++k) my[k] = KEY_INF;
+        LT_FOR(i, B) {
+            const uint32_t ask = a.asks[i];
+            for (int k = 0; k < D; ++k) {
+                const int64_t v = a.a_req[(size_t)k * a.lda + ask];
+                a.sreq[(size_t)i * D + k] = v;
+                const u64 c = v < 0 ? 0ull : (u64)v;
+                my[k] = c < my[k] ? c : my[k];
+            }
+        }
+        for (int k = 0; k < D; ++k) yklt::red_min64(reinterpret_cast<u64*>(&s.minreq[k]), my[k]);
     }
     LT_SYNC();
 
@@ -229,7 +325,7 @@ LT_FN void rounds_stretch(const Args& a, Shared& s) {
             if (sp) a.spent[y] = e;
         }
         LT_SYNC();
-        { int tot; yklt::block_scan(s.scan, s.tmp, lim, &tot); LT_ONE s.keep = tot; LT_SYNC(); }
+        yklt::block_scan(s.scan, s.tmp, lim, &s.keep);   // (the total straight into shared memory: a local's address puts it in local memory)
         LT_FOR(x, lim) {
             const Ent e = a.ord[buf][base + x];
             const bool keep = (x + 1 < lim ? s.scan[x + 1] : (uint32_t)s.keep) != s.scan[x];
@@ -251,6 +347,7 @@ LT_FN void rounds_stretch(const Args& a, Shared& s) {
         W = W < n_act + nl ? W : n_act + nl;
         const int wm = W < n_act ? W : n_act, wl = W < nl ? W : nl;
         LT_ONE { s.m = W; s.n_new = 0; s.keep = 0; }
+        int64_t q[D];   // a candidate's request: D consecutive words of the staged requests, not a gather from the ask table
         {   // ---- S[0, W): the first W entries of order + side list ----
             const Ent* A = a.ord[buf] + hd;
             const u64* lk = s.lk[lb];
@@ -269,16 +366,12 @@ LT_FN void rounds_stretch(const Args& a, Shared& s) {
         }
         // ---- candidates: S[j] for ask t+j ----
         LT_FOR(j, W) {
-            const uint32_t n = (uint32_t)s.er[j];
+            req_of<D>(a, t + j, q);
+            const u64 rn = s.er[j];
+            const uint32_t n = (uint32_t)rn;
             const int64_t* r = a.rec + (size_t)n * RS;
-            int64_t req[D], na[D];
-            const bool ok = accepts_ask<D>(a, r, n, a.asks[t + j], req);
-            u64 key = KEY_INF;
-            if (ok) {
-                for (int k = 0; k < D; ++k) na[k] = r[k] - req[k];
-                key = yklt::key_of<D>(a.policy, a.w, r + D, na);
-            }
-            s.ck[j] = key; s.cr[j] = ok ? s.er[j] : KEY_INF;
+            const bool ok = takes<D>(a, r, n, t + j, q);
+            s.ck[j] = ok ? key_after<D>(a, r, q) : KEY_INF; s.cr[j] = ok ? rn : KEY_INF;
         }
         LT_SYNC();
         LT_PROF(RP_CAND);
@@ -306,10 +399,10 @@ LT_FN void rounds_stretch(const Args& a, Shared& s) {
                 bool stay = false;
                 Ent ne{0, 0};
                 if (j < m) {
+                    req_of<D>(a, t + j, q);   // (reloaded: kept in registers across the prefix minimum, it spills)
                     const uint32_t n = (uint32_t)s.cr[j];
                     int64_t* r = a.rec + (size_t)n * RS;
-                    const uint32_t ask = a.asks[t + j];
-                    for (int k = 0; k < D; ++k) r[k] -= a.a_req[(size_t)k * a.lda + ask];
+                    for (int k = 0; k < D; ++k) r[k] -= q[k];
                     a.res[t + j] = n;
                     ne.key = s.ck[j]; ne.rn = s.cr[j];
                     stay = !spent_of<D>(r, s.minreq);
@@ -322,7 +415,7 @@ LT_FN void rounds_stretch(const Args& a, Shared& s) {
             LT_SYNC();
             LT_PROF(RP_APPLY);
             const int nt = s.n_new;
-            yklt::block_sort_fast(s.tk, s.tr, nt, s.pk, s.pr);
+            sort_new(s.tk, s.tr, nt, s.pk, s.pr);
             LT_PROF(RP_SORT);
             hd += mm; n_act -= mm;
             const u64* ok_ = s.lk[lb] + ml;
@@ -351,15 +444,14 @@ LT_FN void rounds_stretch(const Args& a, Shared& s) {
             LT_ONE s.hit = n_act;
             LT_SYNC();
             Ent* src = a.ord[buf] + hd;
-            const uint32_t ask = a.asks[t];
+            req_of<D>(a, t, q);
             int hit = n_act;
             for (int base = 0; base < n_act && hit == n_act; base += THREADS) {
                 const int lim = n_act - base < THREADS ? n_act - base : THREADS;
                 int my = n_act;
                 LT_FOR(x, lim) {
                     const uint32_t n = (uint32_t)src[base + x].rn;
-                    int64_t req[D];
-                    if (accepts_ask<D>(a, a.rec + (size_t)n * RS, n, ask, req)) my = base + x < my ? base + x : my;
+                    if (takes<D>(a, a.rec + (size_t)n * RS, n, t, q)) my = base + x < my ? base + x : my;
                 }
                 yklt::red_min32(&s.hit, my);
                 LT_SYNC();
@@ -374,12 +466,10 @@ LT_FN void rounds_stretch(const Args& a, Shared& s) {
                     const Ent e = src[hit];
                     const uint32_t n = (uint32_t)e.rn;
                     int64_t* r = a.rec + (size_t)n * RS;
-                    int64_t na[D];
-                    for (int k = 0; k < D; ++k) na[k] = r[k] - a.a_req[(size_t)k * a.lda + ask];
-                    Ent ne; ne.key = yklt::key_of<D>(a.policy, a.w, r + D, na); ne.rn = e.rn;
+                    Ent ne; ne.key = key_after<D>(a, r, q); ne.rn = e.rn;
                     if (ne.key == KEY_INF) s.nan = 1;
                     else {
-                        for (int k = 0; k < D; ++k) r[k] = na[k];
+                        for (int k = 0; k < D; ++k) r[k] -= q[k];
                         a.res[t] = n;
                         if (spent_of<D>(r, s.minreq)) { a.spent[s.n_sp++] = ne; s.n_new = 0; }
                         else { s.tk[0] = ne.key; s.tr[0] = ne.rn; s.n_new = 1; }
@@ -410,7 +500,7 @@ LT_FN void rounds_stretch(const Args& a, Shared& s) {
         const int nt = n_sp - base < WCAP ? n_sp - base : WCAP;
         LT_FOR(x, nt) { const Ent e = a.spent[base + x]; s.tk[x] = e.key; s.tr[x] = e.rn; }
         LT_SYNC();
-        yklt::block_sort_fast(s.tk, s.tr, nt, s.pk, s.pr);
+        sort_new(s.tk, s.tr, nt, s.pk, s.pr);
         merge_into(a.ord[buf] + hd, n_act, 0, 0, s.tk, s.tr, nt, a.ord[buf ^ 1]);
         hd = 0;
         n_act += nt;
@@ -426,6 +516,19 @@ LT_FN void rounds_stretch(const Args& a, Shared& s) {
         a.hdr[R_SPENT] = n_sp;
     }
     LT_SYNC();
+}
+
+template <int D>
+LT_FN void rounds_stretch(const Args& a, Shared& s) {
+#if LT_DEV
+    stretch<D>(a, s);
+#else
+    if (a.sreq) { stretch<D>(a, s); return; }
+    std::vector<int64_t> own((size_t)(a.B > 0 ? a.B : 1) * D);   // a caller that brings no staging buffer
+    Args b = a;
+    b.sreq = own.data();
+    stretch<D>(b, s);
+#endif
 }
 
 }  // namespace ykrd

@@ -1,11 +1,10 @@
 // Host-only emulation of yk_cycle for the CPU test suite: the REAL ordering engine (csrc/yk_orderer.hpp) and the REAL
-// ordered commit (csrc/yk_commit.hpp: epochs, touched-node index, gang roll-back, order merge) driven through the same
-// control flow as csrc/yk_engine.cu (two slots, speculative next batch, rewind, epoch ends) -- only the device part is
-// replaced: the fit rows are computed here by a plain CPU loop over the epoch's sorted view (test infrastructure,
-// never part of the product).  What this cannot cover is the CUDA kernels and the stream plumbing: those are the
-// `-m gpu` tests.
-#include "../../yunikorn_k8shim_b200/csrc/yk_commit.hpp"
-#include "../../yunikorn_k8shim_b200/csrc/yk_orderer.hpp"
+// ordered commit (csrc/yk_commit.hpp: epochs, touched-node index, gang roll-back, order merge) driven by the engine's own
+// batch loop (yk::host_commit in csrc/yk_lattice_host.hpp: two slots, speculative next batch, rewind, epoch ends) -- only
+// the device part is replaced: the fit rows are computed here by a plain CPU loop over the epoch's sorted view, and the
+// speculated fill runs inline (test infrastructure, never part of the product).  What this cannot cover is the CUDA
+// kernels, the stream plumbing and the helper thread: those are the `-m gpu` tests.
+#include "../../yunikorn_k8shim_b200/csrc/yk_lattice_host.hpp"
 #include "shim_tables.hpp"
 
 #include <algorithm>
@@ -206,85 +205,46 @@ static int engine_host_run_impl(
         }
     };
     refresh_view();
-
-    Slot slot[2];
-    size_t bsz = batch;
-    uint32_t n = 0;
-    int rc_over = 0;
-    auto next_batch = [&](Slot& sl, size_t cap_user) {
-        sl.asks.clear();
-        if (cap_user == 0) return;
-        o.fill(bsz, cap_user, sl.asks, sl.snap);
-        if (o.oversize_gang) {
-            if (bsz < batch) { bsz = batch; o.fill(bsz, cap_user, sl.asks, sl.snap); }
-            if (o.oversize_gang) { rc_over = -1; return; }
-        }
-        sweep(sl);
-        if (xrc) rc_over = xrc;
-    };
-    std::vector<uint32_t> result;
-    next_batch(slot[0], max_bindings);
-    if (rc_over) return rc_over;
-    int sc = 0;
-    while (!slot[sc].asks.empty()) {
-        Slot& A = slot[sc];
-        Slot& Nx = slot[sc ^ 1];
-        Nx.asks.clear();
-        const bool room = cm.dirty_list.size() + A.asks.size() < (size_t)epoch_limit;
-        const size_t left = (size_t)max_bindings - n;
-        bool forked = false;
-        if (speculate && room && left > A.asks.size()) { next_batch(Nx, left - A.asks.size()); forked = true; if (rc_over) return rc_over; }
-        size_t consumed = 0;
-        if (nlive == 0) {
-            result.assign(A.asks.size(), yk::CNONE);
-            consumed = ins ? A.asks.size() : std::min<size_t>(1, A.asks.size());
-            if (!ins && !A.asks.empty() && a_gang[A.asks[0]] != yk::CNONE)
-                while (consumed < A.asks.size() && cm.same_gang(A.asks[0], A.asks[consumed])) ++consumed;
-        } else {
-            const int rc = cm.commit_batch(A.asks, A.row_of.data(), A.fit.data(), ins, result, consumed, [&](int) { return (int)A.reps.size(); });
-            if (rc) return rc;
-        }
-        bool failed = false;
-        if (!ins && consumed > 0 && result[consumed - 1] == yk::CNONE) {
-            size_t j = consumed - 1;
-            while (j > 0 && a_gang[A.asks[j]] != yk::CNONE && a_gang[A.asks[j - 1]] == a_gang[A.asks[j]] &&
-                   a_app[A.asks[j - 1]] == a_app[A.asks[j]] && result[j - 1] == yk::CNONE) --j;
-            o.rewind(A.snap, forked ? &Nx.snap : nullptr, A.asks, j);   // also when the speculated batch came out empty
-            failed = true;
-            Nx.asks.clear();
-        }
-        for (size_t i = 0; i < consumed; ++i) {
-            const uint32_t a = A.asks[i];
-            if (result[i] == yk::CNONE) { if (ins) o.fail_in_place(a); continue; }
-            o.confirm(a);
-            out_ask[n] = a; out_node[n] = result[i]; ++n;
-        }
-        bsz = failed ? std::max<size_t>(std::min<size_t>(64, batch), bsz / 4) : std::min<size_t>(batch, bsz * 2);
-        if (Nx.asks.empty() && n < max_bindings) {
-            if (cm.dirty_list.size() * 2 >= (size_t)epoch_limit || failed) {
-                if (!cm.dirty_list.empty() && g_skip_checks) cm.merge_order(order_nodes.data(), nlive);
-                else if (!cm.dirty_list.empty()) {
-                    cm.merge_order(order_nodes.data(), nlive);
-                    // the merged order must be exactly: every node once, ascending by (CURRENT score key, NodeID rank)
-                    std::vector<uint8_t> seen_node(nN, 0);
-                    for (int p = 0; p < nlive; ++p) {
-                        const yk::DirtyRef r = cm.order()[p];
-                        const uint32_t nn = r.node();
-                        if (nn >= nN || seen_node[nn] || order_nodes[p] != nn) return -7;
-                        seen_node[nn] = 1;
-                        yk::NodeView nv = cm.node(nn);
-                        const double sc = yk_node_score(D, policy, weights, nv.total(), nv.avail(), 1);
-                        if (r.key() != yk_key_bits(sc) || r.rank() != n_rank[nn]) return -8;
-                        if (p > 0 && !(cm.order()[p - 1] < r)) return -9;
-                    }
+    // the epoch ends: merge the order, check it (unless g_skip_checks) and refresh the view
+    auto new_epoch = [&]() -> int {
+        if (!cm.dirty_list.empty()) {
+            cm.merge_order(order_nodes.data(), nlive);
+            if (!g_skip_checks) {   // the merged order must be exactly: every node once, ascending by (CURRENT score key, NodeID rank)
+                std::vector<uint8_t> seen_node(nN, 0);
+                for (int p = 0; p < nlive; ++p) {
+                    const yk::DirtyRef r = cm.order()[p];
+                    const uint32_t nn = r.node();
+                    if (nn >= nN || seen_node[nn] || order_nodes[p] != nn) return -7;
+                    seen_node[nn] = 1;
+                    yk::NodeView nv = cm.node(nn);
+                    const double sc = yk_node_score(D, policy, weights, nv.total(), nv.avail(), 1);
+                    if (r.key() != yk_key_bits(sc) || r.rank() != n_rank[nn]) return -8;
+                    if (p > 0 && !(cm.order()[p - 1] < r)) return -9;
                 }
-                refresh_view();
             }
-            next_batch(Nx, (size_t)max_bindings - n);
-            if (rc_over) return rc_over;
         }
-        sc ^= 1;
-    }
+        refresh_view();
+        return 0;
+    };
+
+    // ---- the engine's batch loop (yk::host_commit), speculated fills run inline ----
+    Slot slot[2];
+    uint32_t n = 0;
+    std::vector<uint32_t> result;
+    yk_stats_t st{};
+    size_t bsz = batch;
+    if (!yk::fill_batch(o, bsz, batch, max_bindings, slot[0].asks, slot[0].snap, st)) return -1;
+    yk::HostLoop lp{o, result, nlive == 0, batch, epoch_limit, cm.dirty_list, speculate != 0, max_bindings, n, st, st};
+    const int rc = yk::host_commit(lp, slot,
+                                   [&](Slot& sl, yk_stats_t&) { sweep(sl); return xrc; },
+                                   [&](Slot& sl, std::vector<uint32_t>& res, size_t& consumed) {
+                                       return cm.commit_batch(sl.asks, sl.row_of.data(), sl.fit.data(), ins, res, consumed,
+                                                              [&](int) { return (int)sl.reps.size(); });
+                                   },
+                                   [](auto&& job) { job(); }, [] {}, [](Slot&) { return 0; }, new_epoch,
+                                   [&](uint32_t a, uint32_t node) { out_ask[n] = a; out_node[n] = node; ++n; },
+                                   [](int, const char*) { return -1; });   // the loop's own error: a gang no batch holds
+    if (rc) return rc;
     o.finish();
     *n_out = n;
     if (rows_out) {   // [0] rows swept, then the commit's counters (yk_commit.hpp dbg[]: words scanned, touched candidates walked,

@@ -1,6 +1,7 @@
 """The engine's host side end to end, without a GPU: tests/host/engine_shim.cpp drives the REAL ordering engine
-(csrc/yk_orderer.hpp) and the REAL ordered commit (csrc/yk_commit.hpp) through yk_cycle's control flow -- batches,
-speculative next batch, rewind, epochs with lazy order merges -- with the device sweep replaced by a plain CPU loop.
+(csrc/yk_orderer.hpp) and the REAL ordered commit (csrc/yk_commit.hpp) through yk_cycle's own batch loop
+(yk::host_commit in csrc/yk_lattice_host.hpp) -- batches, speculative next batch, rewind, epochs with lazy order merges --
+with the device sweep replaced by a plain CPU loop.
 Bindings, ask states and node availability must equal the oracle's, for every batch size / epoch length."""
 import ctypes as C
 

@@ -1,7 +1,8 @@
 // yk_commit.hpp -- the ordered commit: turns the fit bitmaps of a batch into bindings that are identical to what the
-// reference's one-allocation-per-pass loop would produce (DESIGN.md "ordered commit").  Host code, no CUDA: the engine
-// (yk_engine.cu) feeds it rows as they arrive from the device; tests/host/engine_shim.cpp feeds it rows computed on
-// the CPU so that this logic -- epochs, the touched-node index, gang roll-back -- is exercised by the CPU test suite.
+// reference's one-allocation-per-pass loop would produce (DESIGN.md "ordered commit").  Host code, no CUDA: both the
+// engine (yk_engine.cu) and tests/host/engine_shim.cpp run it under one batch loop, yk::host_commit (yk_lattice_host.hpp);
+// the engine feeds it rows as they arrive from the device, the shim rows computed on the CPU, so that this logic --
+// epochs, the touched-node index, gang roll-back -- and the loop around it are exercised by the CPU test suite.
 //
 // Invariant it relies on: within an epoch a node that has not been committed to still has exactly the state the sorted
 // view (and therefore the bitmaps) was built from.  For ask i:

@@ -1013,13 +1013,10 @@ int drain(yk_engine* e, Slot& sl) {
 }
 
 // Ordered commit of one batch from its (arriving) bitmaps: the logic is yk::Committer::commit_batch; this wrapper
-// supplies the rows as the read-back chunks land and keeps the timing / counters.
+// supplies the rows as the read-back chunks land and keeps the timing / counters.  Only called while nodes are live.
 int commit(yk_engine* e, Slot& sl, bool insensitive, std::vector<uint32_t>& result, size_t& consumed) {
-    const int B = sl.B;
     const std::vector<uint32_t>& batch = sl.asks;
-    result.assign((size_t)B, YK_NONE);
-    consumed = 0;
-    if (e->ep_rows && e->nlive != 0) {
+    if (e->ep_rows) {
         double t_wait = 0;
         const double t1 = now_ms();
         if (!e->ep_landed) {
@@ -1041,12 +1038,6 @@ int commit(yk_engine* e, Slot& sl, bool insensitive, std::vector<uint32_t>& resu
         e->st.host_ms[3] += t_wait;
         e->st.host_ms[4] += (t2 - t1) - t_wait;
         e->st.commit_ms += (t2 - t1) - t_wait;
-        return YK_OK;
-    }
-    if (e->nlive == 0 || sl.nchunks == 0) {   // no nodes: nothing fits
-        consumed = insensitive ? (size_t)B : std::min<size_t>(1, (size_t)B);
-        if (!insensitive && B > 0 && e->a_gang[batch[0]] != YK_NONE)
-            while (consumed < (size_t)B && e->cm.same_gang(batch[0], batch[consumed])) ++consumed;
         return YK_OK;
     }
     double t_wait = 0;
@@ -1607,16 +1598,11 @@ int run_host(yk_engine* e, Cycle& c) {
         e->epoch_limit = std::max<uint32_t>(e->epoch_limit, 2u * e->nlive);
     rc = begin_epoch(e);
     if (rc) return rc;
-    size_t bsz = e->batch;
-    const size_t bmax = e->batch;
-    const bool ins = e->ord.insensitive;
-    // fill + launch one batch into a slot; B == 0 afterwards means the orderer has nothing (more) to offer
-    auto next_batch = [&](Slot& sl, size_t cap_user, yk_stats_t& st) -> int {
-        const int rcf = fill_batch(e, bsz, bmax, cap_user, sl, st);
-        if (rcf) return rcf;
-        return produce(e, sl, st);
-    };
-    auto merge_worker_stats = [&]() {
+    yk::HostLoop lp{e->ord, c.result, e->nlive == 0, (size_t)e->batch, e->epoch_limit, e->cm.dirty_list, !e->no_spec,
+                    c.max_bindings, c.n, e->st, e->wst};
+    // the speculated fill and launch run on the helper thread into e->wst, merged at the join
+    auto join = [&] {
+        e->worker.wait();
         yk_stats_t& w = e->wst;
         e->st.h2d_bytes += w.h2d_bytes; e->st.d2h_bytes += w.d2h_bytes; e->st.batches += w.batches;
         e->st.asks_swept += w.asks_swept; e->st.rows_swept += w.rows_swept;
@@ -1624,52 +1610,14 @@ int run_host(yk_engine* e, Cycle& c) {
         e->st.host_ms[7] += w.host_ms[2] + w.host_ms[6];   // orderer + launch time hidden behind the commit
         w = yk_stats_t{};
     };
-    int cur = 0;
-    rc = produce(e, e->slot[0], e->st);
-    if (rc) return rc;
-    while (e->slot[cur].B > 0) {
-        Slot& A = e->slot[cur];
-        Slot& Nx = e->slot[cur ^ 1];
-        // speculate the next batch on the same epoch view unless this batch may fill the epoch
-        Nx.asks.clear(); Nx.B = 0; Nx.nchunks = 0;
-        const bool room = e->cm.dirty_list.size() + (size_t)A.B < (size_t)e->epoch_limit;
-        const size_t left = (size_t)c.max_bindings - c.n;
-        bool forked = false;
-        int rc_next = YK_OK;
-        if (room && !e->no_spec && left > (size_t)A.B) {
-            const size_t cap = left - (size_t)A.B;
-            e->worker.submit([&, cap] { rc_next = next_batch(Nx, cap, e->wst); });
-            forked = true;
-        }
-        size_t consumed = 0;
-        rc = commit(e, A, ins, c.result, consumed);
-        if (forked) { e->worker.wait(); merge_worker_stats(); }
-        if (rc) return rc;
-        // the speculated fill is undone even when it produced no batch: it may still have marked asks (headroom skips)
-        const bool failed = yk::settle(e->ord, A.asks, A.snap, forked ? &Nx.snap : nullptr, c.result.data(), consumed, ins, e->st,
-                                       [&](uint32_t a, uint32_t node) { bind_one(e, c, a, node); });
-        if (rc_next) return rc_next;   // this batch's bindings stand; the speculated one never ran
-        if (failed && Nx.B > 0) {   // the speculated batch was built on an order that did not happen: drop it
-            rc = drain(e, Nx);
-            if (rc) return rc;
-            Nx.asks.clear(); Nx.B = 0; Nx.nchunks = 0;
-        }
-        if (failed) { Nx.asks.clear(); Nx.B = 0; Nx.nchunks = 0; }
-        bsz = yk::next_batch_size(bsz, bmax, failed);
-        if (Nx.B == 0 && c.n < c.max_bindings) {
-            // nothing in flight: the epoch may end here (merge order, refresh the device view) before the next batch
-            if (e->cm.dirty_list.size() * 2 >= (size_t)e->epoch_limit || failed) {
-                rc = end_epoch(e, true);
-                if (rc) return rc;
-                rc = begin_epoch(e);
-                if (rc) return rc;
-            }
-            rc = next_batch(Nx, (size_t)c.max_bindings - c.n, e->st);
-            if (rc) return rc;
-        }
-        cur ^= 1;
-    }
-    return YK_OK;
+    return yk::host_commit(lp, e->slot,
+                           [&](Slot& sl, yk_stats_t& st) { return produce(e, sl, st); },
+                           [&](Slot& sl, std::vector<uint32_t>& result, size_t& consumed) { return commit(e, sl, e->ord.insensitive, result, consumed); },
+                           [&](auto&& job) { e->worker.submit(job); }, join,
+                           [&](Slot& sl) { return drain(e, sl); },
+                           [&] { const int rce = end_epoch(e, true); return rce ? rce : begin_epoch(e); },
+                           [&](uint32_t a, uint32_t node) { bind_one(e, c, a, node); },
+                           [&](int code, const char* m) { return e->fail(code, m); });
 }
 
 }  // namespace

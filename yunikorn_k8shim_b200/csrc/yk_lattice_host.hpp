@@ -1,7 +1,10 @@
-// yk_lattice_host.hpp -- host side of the device commit (yk_lattice.h, yk_uniform.h): the per-entry meta words the kernel
-// reads, the test that decides whether a cycle may use the device commit at all, and the driver around the kernels (the
-// batch loop, the segment loop, a uniform run's attempts; settle and fill_batch, which the host commit uses too).  No CUDA
-// in here: csrc/yk_engine.cu drives the kernels with it and tests/host/device_shim.cpp drives their per-item code with it.
+// yk_lattice_host.hpp -- the cycle's two batch loops and the host side of the device commit (yk_lattice.h, yk_uniform.h).
+// yk::host_commit is the host commit's loop (speculation, settle and rewind, batch sizing, epoch ends); yklt::device_commit
+// is the device commit's, around the per-entry meta words the kernel reads, the test that decides whether a cycle may use
+// the device commit at all, the segment loop and a uniform run's attempts.  Both share fill_batch, settle, the batch-size
+// rule and the no-node rule.  No CUDA in here: csrc/yk_engine.cu runs both loops with the sweep and the kernels,
+// tests/host/engine_shim.cpp runs the host loop with a CPU sweep and tests/host/device_shim.cpp the device loop with the
+// kernels' per-item code.
 #pragma once
 #include <chrono>
 #include <cstdint>
@@ -67,6 +70,92 @@ inline bool settle(Orderer& ord, const std::vector<uint32_t>& asks, Orderer::Sna
         st.allocations++;
     }
     return failed;
+}
+
+// Entries of a batch decided when no node is live (nothing fits): all of them in a placement-insensitive order, else the
+// first ask or gang, where the order stops.
+inline size_t no_node_consumed(const Tables& t, const std::vector<uint32_t>& asks, bool ins) {
+    if (ins || asks.empty()) return asks.size();
+    size_t consumed = 1;
+    while (consumed < asks.size() && same_gang(t, asks[0], asks[consumed])) ++consumed;
+    return consumed;
+}
+
+// What the host commit's batch loop works on; the caller owns all of it.
+struct HostLoop {
+    Orderer& ord;
+    std::vector<uint32_t>& result;             // node per entry of the batch being committed, CNONE for none
+    bool no_nodes;
+    size_t bmax;                               // largest batch
+    uint32_t epoch_limit;                      // an epoch ends before its touched-node count would pass this
+    const std::vector<uint32_t>& touched;      // nodes committed to in this epoch (Committer::dirty_list)
+    bool speculate;                            // fill and launch batch k+1 while batch k commits
+    uint32_t max_bindings; const uint32_t& n;  // bindings allowed in the cycle, made so far
+    yk_stats_t& st; yk_stats_t& side_st;       // counters of the loop's thread, of the speculated fill
+};
+
+// The cycle on the host commit, batch by batch; slot[0] holds the first batch, filled and not yet launched.  The slots
+// (SlotT: asks, snap) are the caller's, and so is everything that touches the device or a clock:
+//   launch(slot, stats)              starts the sweep of a filled batch (an empty one included);
+//   commit(slot, result, consumed)   decides one batch into result[0, consumed); only called while nodes are live;
+//   side(job), join()                run job -- the speculated fill and launch -- next to the commit, then wait for it;
+//   drop(slot)                       lets go of a launched batch that will never be committed;
+//   new_epoch()                      ends the epoch (order merge, view refresh) and begins the next one;
+//   bind(ask, node)                  takes a binding (and counts it in lp.n);
+//   fail(yk_status, message)         reports an error.
+// Whether a batch is filled or launched depends only on the orderer, the touched count and the bindings made, which every
+// rank of a multi-GPU cycle shares: the ranks stay in lock-step.
+template <class SlotT, class Launch, class Commit, class Side, class Join, class Drop, class NewEpoch, class Bind, class Fail>
+inline int host_commit(HostLoop& lp, SlotT* slot, Launch&& launch, Commit&& commit, Side&& side, Join&& join, Drop&& drop,
+                       NewEpoch&& new_epoch, Bind&& bind, Fail&& fail) {
+    const bool ins = lp.ord.insensitive;
+    size_t bsz = lp.bmax;
+    // fill + launch one batch into a slot; an empty batch means the orderer has nothing (more) to offer
+    auto next = [&](SlotT& sl, size_t cap_user, yk_stats_t& st) -> int {
+        if (!fill_batch(lp.ord, bsz, lp.bmax, cap_user, sl.asks, sl.snap, st)) return fail(YK_ERR_ARG, GANG_TOO_BIG);
+        return launch(sl, st);
+    };
+    int rc = launch(slot[0], lp.st);
+    if (rc) return rc;
+    for (int cur = 0; !slot[cur].asks.empty(); cur ^= 1) {
+        SlotT& A = slot[cur];
+        SlotT& Nx = slot[cur ^ 1];
+        const size_t B = A.asks.size();
+        // speculate the next batch on the same epoch view unless this batch may fill the epoch
+        Nx.asks.clear();
+        const size_t left = (size_t)lp.max_bindings - lp.n;
+        const bool forked = lp.speculate && lp.touched.size() + B < (size_t)lp.epoch_limit && left > B;
+        int rc_next = 0;
+        if (forked) side([&, cap = left - B] { rc_next = next(Nx, cap, lp.side_st); });
+        size_t consumed = 0;
+        if (lp.no_nodes) {
+            lp.result.assign(B, CNONE);
+            consumed = no_node_consumed(lp.ord.t, A.asks, ins);
+        } else {
+            rc = commit(A, lp.result, consumed);
+        }
+        if (forked) join();
+        if (rc) return rc;
+        // the speculated fill is undone even when it produced no batch: it may still have marked asks (headroom skips)
+        const bool failed = settle(lp.ord, A.asks, A.snap, forked ? &Nx.snap : nullptr, lp.result.data(), consumed, ins, lp.st, bind);
+        if (rc_next) return rc_next;   // this batch's bindings stand; the speculated one never ran
+        if (failed && !Nx.asks.empty()) {   // the speculated batch was built on an order that did not happen: drop it
+            rc = drop(Nx);
+            if (rc) return rc;
+        }
+        if (failed) Nx.asks.clear();
+        bsz = next_batch_size(bsz, lp.bmax, failed);
+        if (Nx.asks.empty() && lp.n < lp.max_bindings) {
+            // nothing in flight: the epoch may end here before the next batch
+            if (lp.touched.size() * 2 >= (size_t)lp.epoch_limit || failed) {
+                rc = new_epoch();
+                if (rc) return rc;
+            }
+            rc = next(Nx, (size_t)lp.max_bindings - lp.n, lp.st);
+            if (rc) return rc;
+        }
+    }
+    return 0;
 }
 
 }  // namespace yk
@@ -386,9 +475,8 @@ inline int device_commit(Loop& lp, Batch&& batch, Bind&& bind, Fail&& fail, bool
         int status = ST_DONE;
         if (lp.no_nodes) {   // nothing fits
             lp.result.assign(B, NONE);
-            consumed = ins ? B : 1;
+            consumed = yk::no_node_consumed(lp.ord.t, lp.asks, ins);
             if (!ins) status = ST_STOPPED;
-            while (!ins && consumed < B && yk::same_gang(lp.ord.t, lp.asks[0], lp.asks[consumed])) ++consumed;
         } else {
             const int rc = batch(B, &status, &consumed);
             if (rc) return rc;

@@ -35,6 +35,7 @@ import "C"
 import (
 	"errors"
 	"fmt"
+	"math"
 	"sort"
 	"strconv"
 	"strings"
@@ -103,6 +104,7 @@ type Engine struct {
 	appQueue []uint32
 	queueIdx map[string]uint32 // "root.a.b" -> index
 	queueLeaf []bool
+	nodeSort nodeSort // what yk_node_sort_set last applied: put back when the rest of a configuration is refused
 	seq      int64
 	stop     chan struct{}
 	kick     chan struct{}
@@ -115,12 +117,13 @@ func New(maxNodes, maxAsks, maxApps, maxQueues int, src ObjectSource) (*Engine, 
 	var cfg C.yk_config
 	cfg.abi_version = C.YK_ABI_VERSION
 	cfg.D = C.uint32_t(len(dims))
-	cfg.policy = C.YK_POLICY_FAIR
-	cfg.weights[0], cfg.weights[1] = 1, 1 // core default node-sort weights: vcore = memory = 1 (SURVEY A.3)
+	// the core's default node sort until the configuration arrives (RegisterResourceManager -> applyConfig -> yk_node_sort_set)
+	ns := defaultNodeSort()
+	cfg.policy, cfg.weights = ns.policy, ns.weights
 	cfg.max_nodes, cfg.max_asks, cfg.max_apps, cfg.max_queues = C.uint32_t(maxNodes), C.uint32_t(maxAsks), C.uint32_t(maxApps), C.uint32_t(maxQueues)
 	cfg.device = -1
 	e := &Engine{src: src, nodeIdx: map[string]uint32{}, askIdx: map[string]uint32{}, appIdx: map[string]uint32{},
-		queueIdx: map[string]uint32{}, stop: make(chan struct{}), kick: make(chan struct{}, 1)}
+		queueIdx: map[string]uint32{}, nodeSort: ns, stop: make(chan struct{}), kick: make(chan struct{}, 1)}
 	if rc := C.yk_create(&cfg, &e.h); rc != C.YK_OK {
 		return nil, errors.New(C.GoString(C.yk_strerror(rc)))
 	}
@@ -150,7 +153,7 @@ func (e *Engine) ck(rc C.int, what string) error {
 
 // ---------------------------------------------------------------------------------------------------------------
 // queues.yaml (the core's configs.SchedulerConfig, schema evidence: test/e2e/framework/helpers/common/
-// test_queues_configs.go:42-60) -> yk_queues_set / yk_queues_priority
+// test_queues_configs.go:42-60) -> yk_queues_set / yk_queues_priority, and the partition's nodesortpolicy -> yk_node_sort_set
 // ---------------------------------------------------------------------------------------------------------------
 
 type queueConf struct {
@@ -160,16 +163,80 @@ type queueConf struct {
 	Properties map[string]string `yaml:"properties"`
 	Queues     []queueConf       `yaml:"queues"`
 }
+
+// the core's configs.NodeSortingPolicy of a partition
+type nodeSortConf struct {
+	Type            string             `yaml:"type"`
+	ResourceWeights map[string]float64 `yaml:"resourceweights"`
+}
 type schedulerConf struct {
 	Partitions []struct {
-		Name            string      `yaml:"name"`
-		Queues          []queueConf `yaml:"queues"`
-		NodeSortPolicy  struct{ Type string `yaml:"type"` } `yaml:"nodesortpolicy"`
+		Name            string       `yaml:"name"`
+		Queues          []queueConf  `yaml:"queues"`
+		NodeSortPolicy  nodeSortConf `yaml:"nodesortpolicy"`
 	} `yaml:"partitions"`
 }
 
 func defaultQueues() []queueConf {
 	return []queueConf{{Name: "root", Parent: true, Queues: []queueConf{{Name: "default"}}}}
+}
+
+// nodeSort is one yk_node_sort_set setting: YK_POLICY_* and the weights in dims order (the rest of [YK_MAX_D] stays 0)
+type nodeSort struct {
+	policy  C.uint32_t
+	weights [C.YK_MAX_D]C.double
+}
+
+// the core's default: fair, vcore = memory = 1 (SURVEY A.3)
+func defaultNodeSort() nodeSort {
+	s := nodeSort{policy: C.YK_POLICY_FAIR}
+	s.weights[0], s.weights[1] = 1, 1
+	return s
+}
+
+// parseNodeSort maps a partition's nodesortpolicy onto the engine's setting.  type: "" (or no block) = fair; "fair" and
+// "binpacking" are exact names; anything else is an error.  resourceweights: absent = the core default; a weight on a
+// resource outside dims (e.g. nvidia.com/gpu) cannot be honoured -- the engine does not track that resource -- so it refuses
+// the configuration rather than sort by something else.
+func parseNodeSort(c nodeSortConf) (nodeSort, error) {
+	s := defaultNodeSort()
+	switch c.Type {
+	case "", "fair":
+	case "binpacking":
+		s.policy = C.YK_POLICY_BINPACKING
+	default:
+		return s, fmt.Errorf("ykgpu: nodesortpolicy type %q: not fair or binpacking", c.Type)
+	}
+	if len(c.ResourceWeights) == 0 {
+		return s, nil
+	}
+	s.weights = [C.YK_MAX_D]C.double{}
+	for name, w := range c.ResourceWeights {
+		k := -1
+		for i, d := range dims {
+			if d == name {
+				k = i
+			}
+		}
+		if k < 0 {
+			return s, fmt.Errorf("ykgpu: nodesortpolicy resourceweights: resource %q is not one the engine sorts by (%s)", name,
+				strings.Join(dims, ", "))
+		}
+		if math.IsNaN(w) || math.IsInf(w, 0) {
+			return s, fmt.Errorf("ykgpu: nodesortpolicy resourceweights: weight of %q is not a finite number", name)
+		}
+		s.weights[k] = C.double(w)
+	}
+	return s, nil
+}
+
+// setNodeSort: yk_node_sort_set refuses (and keeps the old setting) when a present node would score NaN under the new one
+func (e *Engine) setNodeSort(s nodeSort) error {
+	if err := e.ck(C.yk_node_sort_set(e.h, s.policy, &s.weights[0]), "yk_node_sort_set"); err != nil {
+		return err
+	}
+	e.nodeSort = s
+	return nil
 }
 
 // quantity: the core's resources.NewResourceFromConf -- plain integers, "vcore" in milli units when suffixed with m,
@@ -270,7 +337,26 @@ func (e *Engine) applyConfig(cfg string) error {
 		return nil
 	}
 	// one engine = one partition (a second partition is a second Engine on another GPU: DESIGN.md "multi-GPU")
-	return e.setQueues(sc.Partitions[0].Queues)
+	p := sc.Partitions[0]
+	// all or nothing: everything is parsed and validated before the engine changes; the node sort goes first and is put back
+	// when the queue tree is refused, so the shim's old configuration stays in force either way
+	ns, err := parseNodeSort(p.NodeSortPolicy)
+	if err != nil {
+		return err
+	}
+	prev := e.nodeSort
+	if err := e.setNodeSort(ns); err != nil {
+		return err
+	}
+	if err := e.setQueues(p.Queues); err != nil {
+		// the node tables are those the first call saw (e.mu is held throughout): this fails only where prev already made the
+		// cycles fail (a node scoring NaN), and the error then says so
+		if rerr := e.setNodeSort(prev); rerr != nil {
+			return fmt.Errorf("%v; putting the previous node sort back: %v", err, rerr)
+		}
+		return err
+	}
+	return nil
 }
 
 // RegisterResourceManager: pkg/shim/scheduler.go:147-167 hands over the callback object and the queues.yaml text
@@ -286,7 +372,9 @@ func (e *Engine) RegisterResourceManager(req *si.RegisterResourceManagerRequest,
 }
 
 // UpdateConfiguration: a changed queues.yaml.  yk_queues_set refuses a tree that drops a queue applications still sit
-// in (YK_ERR_STATE): the error goes back to the shim, which keeps the old configuration (as the core does).
+// in (YK_ERR_STATE), parseNodeSort an unknown policy or a weight on an untracked resource, yk_node_sort_set a setting under
+// which a node scores NaN: the error goes back to the shim, which keeps the old configuration (as the core does), and so does
+// the engine.  A new nodesortpolicy orders the nodes from the next cycle on.
 func (e *Engine) UpdateConfiguration(req *si.UpdateConfigurationRequest) error {
 	e.mu.Lock()
 	defer e.mu.Unlock()

@@ -13,6 +13,7 @@
  *                                       = common.GetNodeResource, pkg/common/resource.go:188-195
  *   yk_queues_set                       the queues.yaml half of RegisterResourceManager /
  *                                       UpdateConfiguration (pkg/shim/scheduler.go:147-167)
+ *   yk_node_sort_set                    the partition's nodesortpolicy (type, resourceweights) of the same configuration
  *   yk_apps_upsert / yk_apps_remove     SchedulerAPI.UpdateApplication (pkg/cache/application.go:423)
  *   yk_asks_upsert / yk_asks_remove     SchedulerAPI.UpdateAllocation(*si.AllocationRequest) with
  *                                       Allocations without NodeID = asks (pkg/cache/task.go:311-334,
@@ -127,9 +128,10 @@ typedef struct yk_engine yk_engine;
 typedef struct {
     uint32_t abi_version;        /* YK_ABI_VERSION */
     uint32_t D;                  /* resource dimensions 1..YK_MAX_D; by convention 0 vcore(milli) 1 memory 2 pods 3 ephemeral-storage */
-    uint32_t policy;             /* YK_POLICY_* */
+    uint32_t policy;             /* YK_POLICY_*: the initial node sort policy (yk_node_sort_set replaces it) */
     uint32_t batch;              /* asks per sweep batch; 0 = default */
-    double weights[YK_MAX_D];    /* node-sort resource weights; core default vcore=1, memory=1 */
+    double weights[YK_MAX_D];    /* initial node-sort resource weights (yk_node_sort_set replaces them); core default
+                                    vcore=1, memory=1 */
     uint32_t max_nodes, max_asks, max_apps, max_queues;
     int32_t device;              /* CUDA ordinal, -1 = current device */
     uint32_t flags;              /* YK_FLAG_* (0 = defaults) */
@@ -253,6 +255,26 @@ int yk_evaluate(yk_engine* e, uint32_t ask, uint32_t node);
 int yk_evaluate_reserve(yk_engine* e, uint32_t ask, uint32_t node);
 /* node sort keys as the device computes them (float64 score bits), for known-answer tests */
 int yk_node_scores(yk_engine* e, uint32_t n, const uint32_t* idx, double* score_out);
+
+/* Replace the node sort policy and resource weights of a live engine: the partition's nodesortpolicy (type, resourceweights)
+ * of the core's configuration, which the shim hands over in RegisterResourceManager / UpdateConfiguration, after the engine
+ * exists.  weights is [YK_MAX_D]; entries at or beyond D are ignored, exactly as in yk_create.  Takes effect from the next
+ * call that orders or scores nodes (yk_cycle, yk_filter_nodes, yk_preemption_nodes, yk_node_scores).
+ *   Errors: YK_ERR_ARG for a null engine or weights, a policy other than YK_POLICY_FAIR / YK_POLICY_BINPACKING, or a NaN or
+ *     infinite weight among the first D.  Negative weights are accepted, as yk_create accepts them (cycles under them take the
+ *     sweep + host commit).
+ *   All or nothing: before anything changes, every present node is scored on the device under the new setting; if one scores
+ *     NaN (as yk_cycle refuses: e.g. weighted resources with total 0 and non-zero available whose infinite shares cancel), the
+ *     call returns YK_ERR_RANGE and the old setting stays.  With no present node nothing is launched.
+ *   What stays: node tables, ask states, queue / application / user accounting and every counter but other_launches /
+ *     h2d_bytes / d2h_bytes.  Setting the current values again is YK_OK, and the next yk_cycle is the one it would have been.
+ *     The engine keeps no order or key across calls, so the next call behaves exactly as on an engine created with the new
+ *     setting and the same tables.
+ *   Creation-time, not switched: YK_FLAG_BINPACKING_DEVICE, YK_FLAG_HOST_COMMIT / YK_FLAG_DEVICE_COMMIT, D and the capacities.
+ *     An engine created without YK_FLAG_BINPACKING_DEVICE commits binpacking cycles on the host after a switch.
+ *   Multi-GPU split sweep (world > 1): every rank orders the nodes itself, so every rank must make the same call between the
+ *     same two cycles. */
+int yk_node_sort_set(yk_engine* e, uint32_t policy, const double* weights);
 
 /* Every present node's first failing step for a list of asks, in the cycle's node order, evaluated on the device in one
  * grid-wide pass (csrc/yk_filter.cuh).  For the slow-path bridge (walk only the nodes that pass the engine's own steps, in

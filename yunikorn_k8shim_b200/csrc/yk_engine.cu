@@ -21,6 +21,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <cmath>
 #include <mutex>
 #include <new>
 #include <string>
@@ -1905,10 +1906,10 @@ cudaError_t grow(Dev<T>& d, size_t n) { return d.n < n ? d.alloc(n) : cudaSucces
 template <typename T>
 cudaError_t grow(Pin<T>& h, size_t n) { return h.n < n ? h.alloc(n) : cudaSuccess; }
 
-// Enqueue the cycle's node order at this moment (ascending (score, NodeID rank, index)) into f_val_out[0, nlive), with the NaN
-// flag copied to h_f_flag (valid after the stream's next synchronise).  yk_filter_nodes and yk_preemption_nodes use it; its
-// buffers are their own, so a cycle's sort buffers are never touched.  Needs e->nlive > 0 and the tables uploaded.
-int filter_order(yk_engine* e) {
+// Enqueue every present node's sort key under (policy, w) into f_key_in / f_val_in[0, nlive) (NodeID-rank order), with the NaN
+// flag copied to h_f_flag (valid after the stream's next synchronise).  The buffers are the filter's own, so a cycle's sort
+// buffers are never touched.  Needs e->nlive > 0 and the tables uploaded.
+int filter_keys(yk_engine* e, uint32_t policy, const YkWeights& w) {
     cudaStream_t s = e->stream;
     const size_t N = e->maxN;
     const uint32_t nlive = e->nlive;
@@ -1921,13 +1922,24 @@ int filter_order(yk_engine* e) {
         CK(e->f_flag.alloc(1)); CK(e->h_f_flag.alloc(1));
     }
     CK(cudaMemsetAsync(e->f_flag.p, 0, sizeof(int), s));
-    yk_key_kernel<<<(nlive + 255) / 256, 256, 0, s>>>(e->D, e->cfg.policy, e->w, e->d_total.p, e->d_avail.p, e->maxN, e->d_by_rank.p,
+    yk_key_kernel<<<(nlive + 255) / 256, 256, 0, s>>>(e->D, policy, w, e->d_total.p, e->d_avail.p, e->maxN, e->d_by_rank.p,
                                                       (int)nlive, e->f_key_in.p, e->f_val_in.p, e->f_flag.p);
-    size_t tb = e->f_cub_bytes;
-    CK(cub::DeviceRadixSort::SortPairs(e->f_cub.p, tb, e->f_key_in.p, e->f_key_out.p, e->f_val_in.p, e->f_val_out.p, (int)nlive, 0, 64, s));
+    CK(cudaGetLastError());
     CK(cudaMemcpyAsync(e->h_f_flag.p, e->f_flag.p, sizeof(int), cudaMemcpyDeviceToHost, s));
-    e->st.other_launches += 11;   // key + cub radix sort, as device_order
+    e->st.other_launches += 1;
     e->st.d2h_bytes += 4;
+    return YK_OK;
+}
+
+// Enqueue the node order under (policy, w) at this moment (ascending (score, NodeID rank, index)) into f_val_out[0, nlive), with
+// the NaN flag as filter_keys leaves it.  yk_filter_nodes and yk_preemption_nodes use it with the engine's current setting.
+int filter_order(yk_engine* e, uint32_t policy, const YkWeights& w) {
+    const int rc = filter_keys(e, policy, w);
+    if (rc) return rc;
+    size_t tb = e->f_cub_bytes;
+    CK(cub::DeviceRadixSort::SortPairs(e->f_cub.p, tb, e->f_key_in.p, e->f_key_out.p, e->f_val_in.p, e->f_val_out.p, (int)e->nlive, 0, 64,
+                                       e->stream));
+    e->st.other_launches += 10;   // cub radix sort (histogram, exclusive sum, 8 onesweep passes), as device_order
     return YK_OK;
 }
 
@@ -1995,6 +2007,34 @@ int yk_node_scores(yk_engine* e, uint32_t n, const uint32_t* idx, double* out) {
     CK(cudaStreamSynchronize(e->stream));
     memcpy(out, e->h_scores.p, 8 * (size_t)n);
     e->st.other_launches++;
+    return YK_OK;
+}
+
+// Every reader of the setting (the cycle's set-up, commit choice and launches, the queries above) reads e->cfg.policy / e->w
+// when it runs, and the device state kept between cycles (the lattice records and order, the uniform runs' re-keyed order) is
+// rebuilt from the cycle's own initial order: replacing the two here is all a switch needs.
+int yk_node_sort_set(yk_engine* e, uint32_t policy, const double* weights) {
+    if (!e) return YK_ERR_ARG;
+    std::lock_guard<std::mutex> g(e->mu);
+    if (!weights) return e->fail(YK_ERR_ARG, "yk_node_sort_set: null weights");
+    if (policy != YK_POLICY_FAIR && policy != YK_POLICY_BINPACKING) return e->fail(YK_ERR_ARG, "yk_node_sort_set: unknown node sort policy");
+    YkWeights w{};
+    for (int k = 0; k < e->D; ++k) {
+        if (!std::isfinite(weights[k])) return e->fail(YK_ERR_ARG, "yk_node_sort_set: NaN or infinite weight");
+        w.w[k] = weights[k];
+    }
+    int rc = upload_tables(e);
+    if (rc) return rc;
+    if (e->nlive) {   // all or nothing: every present node is scored under the new setting by the cycle's own key kernel first
+        rc = filter_keys(e, policy, w);
+        if (rc) return rc;
+        CK(cudaStreamSynchronize(e->stream));
+        if (e->h_f_flag[0]) return e->fail(YK_ERR_RANGE, "yk_node_sort_set: a present node scores NaN under the new setting (zero total "
+                                                         "on a weighted resource); the old setting is kept");
+    }
+    e->cfg.policy = policy;
+    for (int k = 0; k < 8; ++k) e->cfg.weights[k] = w.w[k];
+    e->w = w;
     return YK_OK;
 }
 
@@ -2066,7 +2106,7 @@ int yk_filter_nodes(yk_engine* e, uint32_t n, const uint32_t* asks, int allocate
     CK(grow(e->f_bits, (size_t)chunk * W)); CK(grow(e->f_tcnt, (size_t)chunk * tiles));
     CK(grow(e->f_counts, (size_t)chunk * YK_FILTER_SLOTS)); CK(grow(e->h_f_counts, (size_t)chunk * YK_FILTER_SLOTS));
     if (k) { CK(grow(e->f_out, (size_t)chunk * k)); CK(grow(e->h_f_out, (size_t)chunk * k)); }
-    rc = filter_order(e);
+    rc = filter_order(e, e->cfg.policy, e->w);
     if (rc) return rc;
 
     YkFilterArgs a{};
@@ -2155,7 +2195,7 @@ int yk_preemption_nodes(yk_engine* e, uint32_t n, const uint32_t* asks, const ui
     const int D = e->D;
     cudaStream_t s = e->stream;
     CK(grow(e->pn_pos, e->maxN));
-    rc = filter_order(e);
+    rc = filter_order(e, e->cfg.policy, e->w);
     if (rc) return rc;
     yk_pn_pos_kernel<<<(nlive + 255) / 256, 256, 0, s>>>(e->f_val_out.p, (int)nlive, e->pn_pos.p);
     CK(cudaGetLastError());

@@ -22,7 +22,7 @@ FILTER_RESERVED = 10
 EXPORTS = [
     "yk_abi_version", "yk_create", "yk_destroy", "yk_nodes_upsert", "yk_nodes_remove", "yk_queues_set", "yk_queues_priority",
     "yk_apps_upsert", "yk_apps_remove", "yk_apps_user", "yk_user_limits_set", "yk_asks_upsert", "yk_asks_remove", "yk_release", "yk_cycle",
-    "yk_ask_states", "yk_nodes_available", "yk_evaluate", "yk_evaluate_reserve", "yk_node_scores", "yk_filter_nodes",
+    "yk_ask_states", "yk_nodes_available", "yk_evaluate", "yk_evaluate_reserve", "yk_node_scores", "yk_node_sort_set", "yk_filter_nodes",
     "yk_preemption_search", "yk_preemption_nodes", "yk_set_exchange",
     "yk_peer_export", "yk_peer_import", "yk_peer_enable", "yk_stats",
     "yk_stats_reset", "yk_strerror", "yk_last_error",
@@ -122,6 +122,18 @@ def _colmajor(x, D, n):
     return np.ascontiguousarray(a)
 
 
+def _node_sort_weights(D, weights):
+    """[8] float64 node-sort weights: None = the core default, vcore = memory = 1 (as far as D reaches)"""
+    w = np.zeros(8)
+    if weights is None:
+        w[0] = 1.0
+        if D > 1:
+            w[1] = 1.0
+    else:
+        w[:len(weights)] = weights
+    return w
+
+
 class Engine:
     """One yk_engine.  Method names and arguments mirror include/ykgpu.h one to one.
 
@@ -136,13 +148,7 @@ class Engine:
         cfg = Config()
         cfg.abi_version = self._lib.yk_abi_version()
         cfg.D, cfg.policy, cfg.batch = D, policy, batch
-        w = np.zeros(8)
-        if weights is None:
-            w[0] = 1.0
-            if D > 1:
-                w[1] = 1.0
-        else:
-            w[:len(weights)] = weights
+        w = _node_sort_weights(D, weights)
         for i in range(8):
             cfg.weights[i] = float(w[i])
         cfg.max_nodes, cfg.max_asks, cfg.max_apps, cfg.max_queues = max_nodes, max_asks, max_apps, max_queues
@@ -295,6 +301,11 @@ class Engine:
         out = np.zeros(idx.size, dtype=np.float64)
         self._ck(self._lib.yk_node_scores(self._h, C.c_uint32(idx.size), _p(idx), _p(out)))
         return out
+
+    def node_sort_set(self, policy, weights=None):
+        """replace the node sort policy and weights of this engine from the next call on; weights=None as in the constructor"""
+        w = _node_sort_weights(self.D, weights)
+        self._ck(self._lib.yk_node_sort_set(self._h, C.c_uint32(policy), w.ctypes.data_as(C.c_void_p)))
 
     def filter_nodes(self, asks, k=0, skip=0, allocate=True):
         """-> (nodes[n][k], n_pass[n], counts[n][FILTER_SLOTS]) uint32: per ask, the passing nodes of pass rank skip .. skip+k-1

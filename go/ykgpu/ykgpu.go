@@ -80,6 +80,8 @@ type askRec struct {
 	foreign   bool   // an occupancy record, not a schedulable ask
 	node      uint32 // foreign / recovered: the node it sits on
 	lastState uint8  // last state reported through UpdateContainerSchedulingState
+	prio      int32  // priority and create_seq as first written: every re-push writes them back
+	seq       int64
 	slow      bool
 	exact     bool // slow only for needsGoPredicates: the dictionary encoded the pod's masks exactly (yk_filter_nodes applies)
 	present   bool
@@ -797,7 +799,7 @@ func (e *Engine) newAskSlot() uint32 {
 	return uint32(len(e.asks) - 1)
 }
 
-// pushAsk (re)writes a pending ask; alloc != nil on the first write (priority, creation time)
+// pushAsk (re)writes a pending ask; alloc != nil on the first write, which fixes its priority and create_seq (creation time)
 func (e *Engine) pushAsk(idx uint32, a *askRec, alloc *si.Allocation) error {
 	var pod *v1.Pod
 	if e.src != nil {
@@ -814,29 +816,67 @@ func (e *Engine) pushAsk(idx uint32, a *askRec, alloc *si.Allocation) error {
 	for k := 0; k < 4; k++ {
 		rq[k] = C.int64_t(a.req[k])
 	}
-	prio, seq := C.int32_t(0), C.int64_t(0)
 	if alloc != nil {
 		created, _ := strconv.ParseInt(alloc.AllocationTags[siCommon.CreationTime], 10, 64)
 		e.seq++
-		prio, seq = C.int32_t(alloc.Priority), C.int64_t(created<<20|e.seq&0xFFFFF) // seconds tie: break by arrival (SURVEY A.6)
+		a.prio, a.seq = alloc.Priority, created<<20|e.seq&0xFFFFF // seconds tie: break by arrival (SURVEY A.6)
 		a.lastState = C.YK_ST_PENDING
 	}
+	prio, seq := C.int32_t(a.prio), C.int64_t(a.seq)
 	i, capp := C.uint32_t(idx), C.uint32_t(app)
 	tol, need, deny, rn, fl := m.tolerated_bits, m.required_bits, m.forbidden_bits, m.required_node, m.flags
 	return e.ck(C.yk_asks_upsert(e.h, 1, &i, &rq[0], &tol, &need, &deny, &prio, &seq, &capp, &rn, &fl, nil), "yk_asks_upsert")
 }
 
 // occupy: a pod that holds resources on a node without being scheduled by this engine -- a foreign pod
-// (context.go:409-472, tagged siCommon.Foreign) or a YuniKorn pod found bound on recovery: the node's availability
-// drops by its request; the release gives it back.
-func (e *Engine) occupy(a *askRec, sign int64) error {
-	n := &e.nodes[a.node]
+// (context.go:409-472, tagged siCommon.Foreign) or a YuniKorn pod found bound on recovery: the node's occupancy grows by
+// d (its request when it arrives, the change of its request on a resize, minus its request on the release) and its
+// availability drops by d, in one node push.
+func (e *Engine) occupy(node uint32, d [4]int64) error {
+	n := &e.nodes[node]
 	var delta [4]int64
 	for k := 0; k < 4; k++ {
-		n.occupied[k] += sign * a.req[k]
-		delta[k] = -sign * a.req[k]
+		n.occupied[k] += d[k]
+		delta[k] = -d[k]
 	}
-	return e.pushNode(a.node, n, delta, false)
+	return e.pushNode(node, n, delta, false)
+}
+
+func neg(v [4]int64) [4]int64 {
+	for k := range v {
+		v[k] = -v[k]
+	}
+	return v
+}
+
+// resize follows an in-place pod resize (KEP-1287): the shim re-sends an allocation under a known key whenever
+// common.GetPodResource of the pod changes (Task.SetTaskPod, task.go:633-647; foreign pods, context.go:427-433).  An
+// unchanged vector is ignored.  A YuniKorn ask, pending or bound, takes the new request in the engine (yk_asks_resize:
+// the bound node, the queues, the application and the user limits follow); a foreign or recovered allocation moves its
+// node's occupancy by the change.
+func (e *Engine) resize(idx uint32, req [4]int64) error {
+	a := &e.asks[idx]
+	if req == a.req {
+		return nil
+	}
+	if a.foreign {
+		var d [4]int64
+		for k := 0; k < 4; k++ {
+			d[k] = req[k] - a.req[k]
+		}
+		a.req = req
+		return e.occupy(a.node, d)
+	}
+	var rq [4]C.int64_t
+	for k := 0; k < 4; k++ {
+		rq[k] = C.int64_t(req[k])
+	}
+	i := C.uint32_t(idx)
+	if err := e.ck(C.yk_asks_resize(e.h, 1, &i, &rq[0]), "yk_asks_resize"); err != nil {
+		return err
+	}
+	a.req = req
+	return nil
 }
 
 // UpdateAllocation: asks are si.Allocation without NodeID (si_helper.go:75-115, sent from task.go:311-334); with a
@@ -851,7 +891,8 @@ func (e *Engine) UpdateAllocation(req *si.AllocationRequest) error {
 		}
 	}
 	for _, al := range req.Allocations {
-		if _, dup := e.askIdx[al.AllocationKey]; dup {
+		if idx, known := e.askIdx[al.AllocationKey]; known {
+			note(e.resize(idx, vec(al.ResourcePerAlloc)))
 			continue
 		}
 		rec := askRec{key: al.AllocationKey, app: al.ApplicationID, req: vec(al.ResourcePerAlloc), present: true}
@@ -865,7 +906,7 @@ func (e *Engine) UpdateAllocation(req *si.AllocationRequest) error {
 			idx := e.newAskSlot()
 			e.asks[idx] = rec
 			e.askIdx[al.AllocationKey] = idx
-			note(e.occupy(&e.asks[idx], +1))
+			note(e.occupy(nidx, rec.req))
 			continue
 		}
 		idx := e.newAskSlot()
@@ -883,7 +924,7 @@ func (e *Engine) UpdateAllocation(req *si.AllocationRequest) error {
 			a := &e.asks[idx]
 			switch {
 			case a.foreign:
-				note(e.occupy(a, -1))
+				note(e.occupy(a.node, neg(a.req)))
 			case a.lastState == C.YK_ST_ALLOCATED:
 				i := C.uint32_t(idx)
 				note(e.ck(C.yk_release(e.h, 1, &i), "yk_release"))

@@ -20,6 +20,8 @@
  *                                       pkg/common/si_helper.go:75-115); ask vector = common.GetPodResource,
  *                                       pkg/common/resource.go:56-109
  *   yk_release                          AllocationRequest.Releases (pkg/cache/task.go:518, context.go:459)
+ *   yk_asks_resize                      UpdateAllocation re-sending a known AllocationKey with a new resource vector: an
+ *                                       in-place pod resize (Task.SetTaskPod, pkg/cache/task.go:633-647)
  *   yk_cycle                            yunikorn-core partition.tryAllocate loop [EXT, SURVEY 3.3] INCLUDING
  *                                       the per-(ask,node) callback ResourceManagerCallback.Predicates
  *                                       (pkg/cache/scheduler_callback.go:196-198 -> pkg/cache/context.go:683-703
@@ -231,6 +233,29 @@ int yk_asks_remove(yk_engine* e, uint32_t a, const uint32_t* idx);
 
 /* give the resources of allocated asks back to their nodes and queues, and forget the asks */
 int yk_release(yk_engine* e, uint32_t n, const uint32_t* ask_idx);
+
+/* Replace the request of present asks, pending or allocated: an in-place pod resize (KEP-1287).  The shim re-sends a task's
+ * allocation with the same AllocationKey whenever common.GetPodResource of its pod changes (Task.SetTaskPod,
+ * pkg/cache/task.go:633-647, from Context.updateYuniKornPod, context.go:341-349); req is the new vector, [D][n].
+ *   Allocated ask (YK_ST_ALLOCATED), delta = new - old: its bound node's available goes down by delta (a node that is no longer
+ *     present is left alone, as yk_release leaves it), and every queue on its application's chain, the application's
+ *     allocation and the user-limit held entries that apply go up by delta; yk_release later gives back the new request.
+ *     Nothing is checked against fit, headroom or limits: the kubelet has applied the resize already (an infeasible one never
+ *     arrives: GetPodResource then reports the status requests).  A node may so end up with negative available (every path
+ *     treats it as 0), a queue over its max or a user over a limit (their later asks are SKIPPED).
+ *   Any other present ask (pending, NOFIT, SKIPPED, INVALID, SLOWPATH): the request is replaced, the ask is signed again and
+ *     its cause follows the new request (not strictly greater than zero: INVALID from the next cycle, and valid again after a
+ *     later resize).  Priority, create_seq, application, masks, required node, flags and gang stay, and so does its place in
+ *     the order; the next cycle is the one yk_asks_upsert with the same other fields would give.  Its state stays what the
+ *     last cycle left until the next cycle.
+ *   Errors, all checked before anything changes; nothing changes on an error:
+ *     YK_ERR_ARG   idx / req NULL with n > 0, an index >= max_asks, the same index twice, a negative entry for an allocated ask;
+ *     YK_ERR_STATE an ask that is not present;
+ *     YK_ERR_RANGE a sum that would overflow int64 (a node's available, a queue's, application's or user's allocation).
+ *   n == 0 and an unchanged vector are YK_OK, and the next cycle is unchanged.  No counter moves and nothing is launched; the
+ *   node and ask tables are uploaded by the next call that reads them.  Multi-GPU split sweep (world > 1): every rank makes
+ *   the same call between the same two cycles. */
+int yk_asks_resize(yk_engine* e, uint32_t n, const uint32_t* idx, const int64_t* req /* [D][n] column-major */);
 
 /* One scheduling cycle: runs schedule() passes until no pending ask can be placed or max_bindings is
  * reached.  out[0..*n_out) are the bindings in the reference's commit order.  slow_path_asks (may be NULL)

@@ -1087,17 +1087,62 @@ static bool contiguous_run(const uint32_t* idx, uint32_t n) {
     for (uint32_t i = 1; i < n; ++i) if (idx[i] != idx[0] + i) return false;
     return n > 0;
 }
-// what the user of application p holds under every limit entry that applies to it moves by sign * request(ask)
-static void user_held_add(yk_engine* e, uint32_t p, uint32_t ask, int sign) {
+// Every int64 sum that allocated ask a is counted in, as f(k, sum, sign) for dimension k: its bound node's available
+// (sign -1; only while the node is present, and only with `node`), then +1 for every queue on its application's chain, the
+// application, and the user-limit entries that apply to the application's user.  The one definition of what an allocation
+// is accounted in: alloc_move and alloc_move_fits walk it.
+template <typename F>
+static void alloc_sums(yk_engine* e, uint32_t a, bool node, F&& f) {
+    const uint32_t n = e->a_bound[a], p = e->a_app[a];
+    for (int k = 0; k < e->D; ++k) {
+        if (node && n != YK_NONE && e->n_present[n]) f(k, e->n_avail[(size_t)k * e->maxN + n], -1);
+        for (uint32_t q = e->p_queue[p]; q != YK_NONE; q = e->q_parent[q]) f(k, e->q_alloc[(size_t)k * e->nq + q], +1);
+        f(k, e->p_alloc[(size_t)k * e->maxP + p], +1);
+    }
     if (!e->n_ul || e->p_user[p] == YK_NONE) return;
     for (uint32_t l = 0; l < e->n_ul; ++l) {
         if (e->ul_user[l] != e->p_user[p]) continue;
         for (uint32_t q = e->p_queue[p]; q != YK_NONE; q = e->q_parent[q])
             if (q == e->ul_queue[l]) {
-                for (int k = 0; k < e->D; ++k) e->ul_alloc[(size_t)k * e->n_ul + l] += sign * e->a_req[(size_t)k * e->maxA + ask];
+                for (int k = 0; k < e->D; ++k) f(k, e->ul_alloc[(size_t)k * e->n_ul + l], +1);
                 break;
             }
     }
+}
+// allocated ask a's holdings move by d[0, D): the node's available by -d, the queues, application and user entries by +d
+static void alloc_move(yk_engine* e, uint32_t a, const int64_t* d, bool node = true) {
+    alloc_sums(e, a, node, [d](int k, int64_t& s, int sign) { s += sign * d[k]; });
+}
+// whether alloc_move(e, a, d) keeps every sum inside int64
+static bool alloc_move_fits(yk_engine* e, uint32_t a, const int64_t* d) {
+    bool ok = true;
+    alloc_sums(e, a, true, [&](int k, int64_t& s, int sign) {
+        int64_t r;
+        ok = ok && !(sign > 0 ? __builtin_add_overflow(s, d[k], &r) : __builtin_sub_overflow(s, d[k], &r));
+    });
+    return ok;
+}
+// ask x's request is what it is, in d[0, D)
+static void ask_request(const yk_engine* e, uint32_t x, int64_t* d) {
+    for (int k = 0; k < e->D; ++k) d[k] = e->a_req[(size_t)k * e->maxA + x];
+}
+// ask x's predicate inputs (request, masks, node) and flags were just rewritten: its signature hash, signature number and
+// cause follow.  The number x represented is retired, so asks still holding it stay equal among themselves.
+static void ask_resign(yk_engine* e, const yk::CommitTables& sv, uint32_t x) {
+    e->a_sig[x] = yk::ask_signature(sv, x);
+    e->sigs.retire(x);
+    if (e->sigs.n > 2 * e->maxA) {   // too many stale numbers: renumber the present asks
+        e->sigs.reset(e->maxA);
+        for (uint32_t y = 0; y < e->a_hi; ++y) if (y != x && e->a_state[y] != yk::ST_ABSENT) e->a_sigid[y] = e->sigs.get(sv, e->a_sig[y], y);
+    }
+    e->a_sigid[x] = e->sigs.get(sv, e->a_sig[x], x);
+    e->a_cause[x] = yk::ask_cause(e->D, e->a_req.p, e->maxA, e->a_flags.data(), x);
+}
+// just enough of a view of the ask tables for the signature hash
+static yk::CommitTables sig_view(yk_engine* e) {
+    yk::CommitTables sv;
+    sv.D = e->D; sv.lda = e->maxA; sv.a_req = e->a_req.p; sv.a_tol = e->a_tol.p; sv.a_need = e->a_need.p; sv.a_deny = e->a_deny.p; sv.a_node = e->a_node.p;
+    return sv;
 }
 
 template <typename T>
@@ -1441,8 +1486,7 @@ int yk_asks_upsert(yk_engine* e, uint32_t a, const uint32_t* idx, const int64_t*
             return e->fail(YK_ERR_ARG, "yk_asks_upsert: required_node beyond max_nodes");
         if (e->a_state[idx[i]] == yk::ST_ALLOCATED) return e->fail(YK_ERR_STATE, "yk_asks_upsert: ask holds an allocation (release it first)");
     }
-    yk::CommitTables sv;   // just enough of a view for the signature hash
-    sv.D = e->D; sv.lda = e->maxA; sv.a_req = e->a_req.p; sv.a_tol = e->a_tol.p; sv.a_need = e->a_need.p; sv.a_deny = e->a_deny.p; sv.a_node = e->a_node.p;
+    const yk::CommitTables sv = sig_view(e);
     if (contiguous_run(idx, a)) {   // whole-column copies, then the signature hashes in one sequential pass
         const uint32_t x0 = idx[0];
         for (int k = 0; k < e->D; ++k) memcpy(&e->a_req[(size_t)k * e->maxA + x0], req + (size_t)k * a, sizeof(int64_t) * (size_t)a);
@@ -1480,22 +1524,15 @@ int yk_asks_upsert(yk_engine* e, uint32_t a, const uint32_t* idx, const int64_t*
         e->a_need[x] = need ? need[i] : 0;
         e->a_deny[x] = deny ? deny[i] : 0;
         e->a_node[x] = required_node ? required_node[i] : YK_NONE;
-        e->a_sig[x] = yk::ask_signature(sv, x);
-        e->sigs.retire(x);
-        if (e->sigs.n > 2 * e->maxA) {   // too many stale numbers: renumber the present asks
-            e->sigs.reset(e->maxA);
-            for (uint32_t y = 0; y < e->a_hi; ++y) if (y != x && e->a_state[y] != yk::ST_ABSENT) e->a_sigid[y] = e->sigs.get(sv, e->a_sig[y], y);
-        }
-        e->a_sigid[x] = e->sigs.get(sv, e->a_sig[x], x);
         e->a_prio[x] = prio ? prio[i] : 0;
         e->a_create[x] = create_seq[i];
         e->a_app[x] = app[i];
         e->a_flags[x] = flags ? flags[i] : 0;
-        e->a_cause[x] = yk::ask_cause(e->D, e->a_req.p, e->maxA, e->a_flags.data(), x);
         e->a_gang[x] = gang ? gang[i] : YK_NONE;
         e->a_state[x] = yk::ST_PENDING;
         e->a_bound[x] = YK_NONE;
         e->a_hi = std::max(e->a_hi, x + 1);
+        ask_resign(e, sv, x);
     }
     e->asks_stale = true;
     return YK_OK;
@@ -1520,18 +1557,66 @@ int yk_release(yk_engine* e, uint32_t n, const uint32_t* idx) {
     for (uint32_t i = 0; i < n; ++i)
         if (idx[i] >= e->maxA || e->a_state[idx[i]] != yk::ST_ALLOCATED) return e->fail(YK_ERR_STATE, "yk_release: ask holds no allocation");
     for (uint32_t i = 0; i < n; ++i) {
-        const uint32_t a = idx[i], node = e->a_bound[a];
-        for (int k = 0; k < e->D; ++k) {
-            const int64_t r = e->a_req[(size_t)k * e->maxA + a];
-            if (node != YK_NONE && e->n_present[node]) e->n_avail[(size_t)k * e->maxN + node] += r;
-            for (uint32_t q = e->p_queue[e->a_app[a]]; q != YK_NONE; q = e->q_parent[q]) e->q_alloc[(size_t)k * e->nq + q] -= r;
-            e->p_alloc[(size_t)k * e->maxP + e->a_app[a]] -= r;
-        }
-        user_held_add(e, e->a_app[a], a, -1);
+        const uint32_t a = idx[i];
+        int64_t d[8];
+        ask_request(e, a, d);
+        for (int k = 0; k < e->D; ++k) d[k] = -d[k];
+        alloc_move(e, a, d);
         e->a_state[a] = yk::ST_ABSENT;
         e->a_bound[a] = YK_NONE;
     }
     e->nodes_stale = true;
+    return YK_OK;
+}
+
+int yk_asks_resize(yk_engine* e, uint32_t n, const uint32_t* idx, const int64_t* req) {
+    if (!e) return YK_ERR_ARG;
+    std::lock_guard<std::mutex> g(e->mu);
+    if (n && (!idx || !req)) return e->fail(YK_ERR_ARG, "yk_asks_resize: null array");
+    const int D = e->D;
+    std::vector<uint32_t> sorted(idx, idx + n);
+    std::sort(sorted.begin(), sorted.end());
+    for (uint32_t i = 0; i < n; ++i) {
+        if (sorted[i] >= e->maxA) return e->fail(YK_ERR_ARG, "yk_asks_resize: index beyond max_asks");
+        if (i && sorted[i] == sorted[i - 1]) return e->fail(YK_ERR_ARG, "yk_asks_resize: the same ask twice");
+    }
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t x = idx[i];
+        if (e->a_state[x] == yk::ST_ABSENT) return e->fail(YK_ERR_STATE, "yk_asks_resize: ask not present");
+        if (e->a_state[x] == yk::ST_ALLOCATED)
+            for (int k = 0; k < D; ++k)
+                if (req[(size_t)k * n + i] < 0) return e->fail(YK_ERR_ARG, "yk_asks_resize: negative request for an allocated ask");
+    }
+    // allocations first: each moves by new - old, checked against overflow before it is applied; on an overflow the ones
+    // already moved are moved back (exact: they return to the values they had), so nothing has changed
+    std::vector<int64_t> delta((size_t)n * D);
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t x = idx[i];
+        if (e->a_state[x] != yk::ST_ALLOCATED) continue;
+        int64_t* d = &delta[(size_t)i * D];
+        for (int k = 0; k < D; ++k) d[k] = req[(size_t)k * n + i] - e->a_req[(size_t)k * e->maxA + x];   // both >= 0
+        if (alloc_move_fits(e, x, d)) { alloc_move(e, x, d); continue; }
+        for (uint32_t j = i; j-- > 0;) {
+            if (e->a_state[idx[j]] != yk::ST_ALLOCATED) continue;
+            int64_t back[8];
+            for (int k = 0; k < D; ++k) back[k] = -delta[(size_t)j * D + k];
+            alloc_move(e, idx[j], back);
+        }
+        return e->fail(YK_ERR_RANGE, "yk_asks_resize: a node's available or a queue's, application's or user's allocation would overflow int64");
+    }
+    // then the requests; an ask whose vector changed is signed again and gets its cause from the new request
+    const yk::CommitTables sv = sig_view(e);
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t x = idx[i];
+        bool same = true;
+        for (int k = 0; k < D; ++k) {
+            int64_t& r = e->a_req[(size_t)k * e->maxA + x];
+            same = same && r == req[(size_t)k * n + i];
+            r = req[(size_t)k * n + i];
+        }
+        if (!same) ask_resign(e, sv, x);
+    }
+    if (n) e->nodes_stale = e->asks_stale = true;
     return YK_OK;
 }
 
@@ -1855,14 +1940,10 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
         e->worker.wait();
         for (Slot& sl : e->slot) { if (sl.B > 0 && sl.nchunks > 0) cudaEventSynchronize(sl.ev[(size_t)sl.nchunks - 1]); sl.asks.clear(); sl.B = 0; sl.nchunks = 0; }
         for (uint32_t a : pending) if (e->a_state[a] == yk::ST_TENTATIVE) e->a_state[a] = yk::ST_PENDING;
-        for (uint32_t i = 0; i < c.n; ++i) {
-            const uint32_t a = out[i].ask;
-            for (int k = 0; k < e->D; ++k) {
-                const int64_t r = e->a_req[(size_t)k * e->maxA + a];
-                for (uint32_t q = e->p_queue[e->a_app[a]]; q != YK_NONE; q = e->q_parent[q]) e->q_alloc[(size_t)k * e->nq + q] += r;
-                e->p_alloc[(size_t)k * e->maxP + e->a_app[a]] += r;
-            }
-            user_held_add(e, e->a_app[a], a, +1);
+        for (uint32_t i = 0; i < c.n; ++i) {   // (the commit has already taken them from their nodes)
+            int64_t r[8];
+            ask_request(e, out[i].ask, r);
+            alloc_move(e, out[i].ask, r, false);
         }
     } else {
         e->ord.finish();

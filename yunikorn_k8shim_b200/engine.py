@@ -21,7 +21,8 @@ FILTER_RESERVED = 10
 
 EXPORTS = [
     "yk_abi_version", "yk_create", "yk_destroy", "yk_nodes_upsert", "yk_nodes_remove", "yk_queues_set", "yk_queues_priority",
-    "yk_apps_upsert", "yk_apps_remove", "yk_apps_user", "yk_user_limits_set", "yk_asks_upsert", "yk_asks_remove", "yk_release", "yk_cycle",
+    "yk_apps_upsert", "yk_apps_remove", "yk_apps_user", "yk_user_limits_set", "yk_asks_upsert", "yk_asks_remove", "yk_release",
+    "yk_asks_resize", "yk_cycle",
     "yk_ask_states", "yk_nodes_available", "yk_evaluate", "yk_evaluate_reserve", "yk_node_scores", "yk_node_sort_set", "yk_filter_nodes",
     "yk_preemption_search", "yk_preemption_nodes", "yk_set_exchange",
     "yk_peer_export", "yk_peer_import", "yk_peer_enable", "yk_stats",
@@ -265,6 +266,12 @@ class Engine:
     def release(self, ask_idx):
         idx = _arr(ask_idx, np.uint32)
         self._ck(self._lib.yk_release(self._h, C.c_uint32(idx.size), _p(idx)))
+
+    def asks_resize(self, idx, req):
+        """new requests for present asks, pending or allocated (an in-place pod resize); req as in asks_upsert"""
+        idx = _arr(idx, np.uint32)
+        n = idx.size
+        self._ck(self._lib.yk_asks_resize(self._h, C.c_uint32(n), _p(idx), _p(_colmajor(req, self.D, n))))
 
     # ---- the cycle ----
     def cycle(self, max_bindings, slow_cap=0):

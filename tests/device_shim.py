@@ -15,11 +15,12 @@ from test_engine_host import run_engine_host
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 INELIGIBLE = 100     # binpacking without the flag, negative weighted totals, duplicate NodeID ranks, mixed gangs
+HOST_COMMIT = 101    # auto=True: the engine's choice starts the cycle on the host commit (nothing committed)
 YK_ERR_RANGE = -5    # a NaN node score
 # the device shim's counters, in its stats_out order
 STATS = ("subruns", "fullscans", "sorts", "elems", "quick", "escalations", "handoffs", "batches", "uniform_attempts",
          "uniform_retries", "uniform_asks", "uniform_runs", "uniform_elements", "passes", "singles", "round_asks",
-         "round_stretches", "parked")
+         "round_stretches", "parked", "device")
 
 
 @functools.cache
@@ -37,15 +38,17 @@ def dshim():
     return load("device_shim")
 
 
-def run(shim, s, rounds=1, binpacking=0, uniform=(0, 0), window=0, guard=-1, stats=None, **kw):
+def run(shim, s, rounds=1, binpacking=0, uniform=(0, 0), window=0, guard=-1, round_min=-1, auto=False, stats=None, **kw):
     """one cycle of snapshot s on the device shim -> run_engine_host's (rc, ask, node, state, avail).  The engine's knobs:
-    rounds 1 is `auto`'s routing (round-eligible stretches on the round commit), 0 forced `device` (the lattice kernel
-    takes every stretch); binpacking 1 is YK_FLAG_BINPACKING_DEVICE; uniform = (shortest uniform run, first depth), 0 =
-    off / the engine's rule; window and guard of the round commit, 0 / < 0 = the engine's.  `stats`, a list, gets the
-    counters by name."""
-    shim.host_set_device(C.c_int(rounds), C.c_int(binpacking))
+    auto is the engine's `auto` (its commit choice, first batch and routing; HOST_COMMIT when the cycle starts on the host
+    commit); otherwise the forced `device` choice at `batch`, where rounds 1 is `auto`'s routing (round-eligible stretches
+    on the round commit) and 0 forced `device`'s (the lattice kernel takes every stretch); binpacking 1 is
+    YK_FLAG_BINPACKING_DEVICE; uniform = (shortest uniform run, first depth), 0 = off / the engine's rule; window, guard and
+    round_min (YK_ROUND_MIN) of the round commit, 0 / < 0 / < 0 = the engine's.  `stats`, a list, gets the counters by
+    name."""
+    shim.host_set_device(C.c_int(rounds), C.c_int(binpacking), C.c_int(auto))
     shim.host_set_uniform(C.c_int(uniform[0]), C.c_int(uniform[1]))
-    shim.host_set_rounds(C.c_int(window), C.c_int(guard))
+    shim.host_set_rounds(C.c_int(window), C.c_int(guard), C.c_int(round_min))
     rows = []
     r = run_engine_host(shim, s, fn="device_host_run", rows=rows, **kw)
     if stats is not None:

@@ -2,7 +2,8 @@
 // source -- nvcc turns them into the lattice, round and uniform-run kernels, g++ turns the SAME code into plain loops -- so
 // the device commit (lattice sub-runs, rounds, uniform-run attempts, binpacking fills) is checked against the oracle here
 // without a GPU.  The driver around them is the engine's own: the ordering engine (csrc/yk_orderer.hpp) and, from
-// csrc/yk_lattice_host.hpp, eligibility, the batch loop, the segment loop, a uniform run's attempts and the per-batch routing.
+// csrc/yk_lattice_host.hpp, the commit choice, the batch loop, the segment loop, a uniform run's attempts and the per-batch
+// routing.
 // std::stable_sort stands in for the cub radix sorts and a sequential sum for the cub scan.  After every kernel stand-in the
 // shim checks that the node order is exactly "every node once, ascending by (current key, NodeID rank)".
 //
@@ -18,16 +19,21 @@
 #include <memory>
 #include <vector>
 
-// the engine's commit choice: rounds = 1 routes round-eligible stretches to the round commit (`auto`), 0 leaves every
-// stretch to the lattice kernel (forced `device`); binpacking = 1 is YK_FLAG_BINPACKING_DEVICE
-static int g_rounds = 1, g_binpacking = 0;
-extern "C" void host_set_device(int rounds, int binpacking) { g_rounds = rounds; g_binpacking = binpacking; }
+// the engine's commit choice: automatic = 1 is `auto` (yklt::choose_commit's cost rule picks the commit and cuts the first
+// batch; a cycle it leaves on the host commit returns HOST_COMMIT uncommitted); otherwise the forced `device` choice, with
+// batches cut at `batch`, where rounds = 1 routes round-eligible stretches to the round commit as `auto` does and 0 leaves
+// every stretch to the lattice kernel; binpacking = 1 is YK_FLAG_BINPACKING_DEVICE
+static int g_rounds = 1, g_binpacking = 0, g_auto = 0;
+extern "C" void host_set_device(int rounds, int binpacking, int automatic) { g_rounds = rounds; g_binpacking = binpacking; g_auto = automatic; }
 // shortest uniform run that takes the uniform-run path (0: never), and how deep the first attempt generates (0: the engine's rule)
 static int g_un_min = 0, g_un_depth = 0;
 extern "C" void host_set_uniform(int min_run, int first_depth) { g_un_min = min_run; g_un_depth = first_depth; }
-// candidates per round (0: ykrd::WCAP) and the guard's asks per pass (< 0: the engine's value)
-static int g_rd_window = 0, g_rd_guard = -1;
-extern "C" void host_set_rounds(int window, int guard) { g_rd_window = window; g_rd_guard = guard; }
+// candidates per round (0: ykrd::WCAP), the guard's asks per pass and the fewest pending asks for which a mask-free cycle
+// starts on the round commit under `auto` (YK_ROUND_MIN; < 0: the engine's values)
+static int g_rd_window = 0, g_rd_guard = -1, g_rd_min = -1;
+extern "C" void host_set_rounds(int window, int guard, int min_asks) { g_rd_window = window; g_rd_guard = guard; g_rd_min = min_asks; }
+
+constexpr int INELIGIBLE = 100, HOST_COMMIT = 101;
 
 namespace {
 
@@ -54,14 +60,31 @@ int run_d(uint32_t policy, const double* weights,
     yk::CommitTables ct;
     ct.D = D; ct.policy = policy; ct.w = weights; ct.lda = nA;
     ct.a_req = a_req; ct.a_tol = a_tol; ct.a_need = a_need; ct.a_deny = a_deny; ct.a_node = a_node; ct.a_gang = a_gang; ct.a_app = a_app;
-    const std::vector<uint8_t> npresent(nN, 1);
-    if (!yklt::eligible(ct, nN, npresent.data(), n_total, nN, n_rank, pending, nullptr, nullptr, g_binpacking != 0).ok) return 100;
     std::vector<uint64_t> a_sig(nA);
     std::vector<uint32_t> a_shape(nA, 0), a_sigid(nA, 0);
     for (uint32_t a = 0; a < nA; ++a) a_sig[a] = yk::ask_signature(ct, a);
-    uint32_t n_shapes = 0;
-    yklt::assign_shapes(ct, pending, a_shape, &n_shapes);
     yklt::assign_sigs(ct, a_sig.data(), pending, a_sigid);
+
+    // the engine's commit choice on every node live and every ask pending, in index order; the forced choice fills the first
+    // batch at `batch` (the largest batch stands in for the whole static order)
+    const bool automatic = g_auto && g_un_min > 0 && (policy == YK_POLICY_FAIR || g_binpacking);
+    uint64_t taints = 0;
+    for (uint32_t nn = 0; nn < nN; ++nn) taints |= n_taint[nn];
+    yklt::Scan scan;
+    scan.taints = taints;
+    if (automatic) for (uint32_t a : pending) scan.add(ct, a_sigid.data(), a);
+    scan.done(ct, pending, !g_auto, a_shape);
+    std::vector<uint32_t> asks, result, meta(std::max<uint32_t>(nA, 1)), shp(meta.size()), sig(meta.size());
+    std::vector<ykun::Segment> segs;
+    yk::Orderer::Snap snap;
+    yk_stats_t st{};
+    const std::vector<uint8_t> npresent(nN, 1);
+    const yklt::ChoiceIn in{o, ct, pending, nN, npresent.data(), n_total, nN, n_rank, nullptr, nullptr, !g_auto, automatic,
+                            g_binpacking != 0, g_un_min, g_rd_min >= 0 ? g_rd_min : yklt::RD_MIN, scan, batch, g_auto ? nA : batch,
+                            max_bindings, a_shape.data(), a_sigid.data(), asks, snap, meta.data(), shp.data(), sig.data(), segs, st};
+    yklt::Choice choice;
+    if (!yklt::choose_commit(in, choice)) return -1;
+    if (!choice.device) return g_auto ? HOST_COMMIT : INELIGIBLE;
 
     // ---- device state: node records and the order (what yk_key_kernel + the radix sort + yk_lt_init_kernel build) ----
     const int RS = yklt::record_words(D);
@@ -138,8 +161,6 @@ int run_d(uint32_t policy, const double* weights,
 
     // a uniform run: the engine's attempt loop (ykun::uniform_run) with the kernels of yk_uniform.cuh replaced by loops over
     // the same per-item bodies -- lt_uniform's choice: a binpacking fill (un_fill) or a depth attempt (un_attempt)
-    std::vector<uint32_t> asks, result, meta(std::max<uint32_t>(nA, 1)), shp(meta.size()), sig(meta.size());
-    yk_stats_t st{};
     uint64_t attempts = 0;
     std::vector<uint32_t> byrank(nN);   // the nodes by ascending (NodeID rank, index)
     for (uint32_t i = 0; i < nN; ++i) byrank[i] = i;
@@ -210,8 +231,6 @@ int run_d(uint32_t policy, const double* weights,
         return *status == yklt::ST_NAN || order_ok() ? 0 : -9;
     };
     // a round-eligible stretch: yk_rounds_kernel's body as plain loops
-    uint64_t taints = 0;
-    for (uint32_t nn = 0; nn < nN; ++nn) taints |= n_taint[nn];
     std::vector<yklt::Ent> spent(std::max<uint32_t>(nN, 1));
     std::unique_ptr<ykrd::Shared> rs(new ykrd::Shared());
     int rhdr[ykrd::R_WORDS] = {0, 0, 0, 0, 0};
@@ -231,10 +250,9 @@ int run_d(uint32_t policy, const double* weights,
         passes += (uint64_t)rhdr[ykrd::R_PASSES]; parked += (uint64_t)rhdr[ykrd::R_SPENT]; singles += (uint64_t)rhdr[ykrd::R_SINGLES]; round_asks += *consumed; ++round_stretches;
         return *status == yklt::ST_NAN || order_ok() ? 0 : -9;
     };
-    std::vector<ykun::Segment> segs;
     auto device_batch = [&](size_t B, int* status, size_t* consumed) -> int {
         result.assign(B, yk::CNONE);
-        return yklt::route_batch(bp, g_rounds != 0, ct, ins, taints, asks.data(), segs, meta.data(), uniform, rounds, window, status, consumed);
+        return yklt::route_batch(bp, g_auto || g_rounds != 0, ct, ins, taints, asks.data(), segs, meta.data(), uniform, rounds, window, status, consumed);
     };
     // after a hand-off: a plain sequential first fit with gang roll-back, the stand-in for the engine's host commit
     auto sequential = [&](size_t B, int* status, size_t* consumed) -> int {
@@ -265,16 +283,13 @@ int run_d(uint32_t policy, const double* weights,
     // is -13 in an insensitive order, -12 in a placement-sensitive one
     auto fail = [&](int code, const char*) { return code == YK_ERR_CUDA ? (ins ? -13 : -12) : code; };
 
-    yk::Orderer::Snap snap;
-    bool plan_ready = false, handoff = false;
-    yklt::Loop lp{o, ct, a_shape.data(), a_sigid.data(), asks, snap, result, meta.data(), shp.data(), sig.data(), segs, plan_ready,
-                  yklt::min_run(bp, g_un_min), nN == 0, batch, max_bindings, n, st};
-    size_t bsz = batch;
-    if (!yk::fill_batch(o, bsz, batch, max_bindings, asks, snap, st)) return -1;
+    bool handoff = false;
+    yklt::Loop lp{o, ct, choice.shape_ids, a_sigid.data(), asks, snap, result, meta.data(), shp.data(), sig.data(), segs,
+                  choice.plan_ready, yklt::min_run(bp, g_un_min), nN == 0, ins ? (size_t)in.maxA : batch, max_bindings, n, st};
     int rc = yklt::device_commit(lp, device_batch, bind, fail, handoff);
     if (!rc && handoff) {   // the engine's path: the rest of the cycle on the host commit, never back on the device
         lp.min_run = 0;
-        bsz = batch;
+        size_t bsz = batch;
         if (!yk::fill_batch(o, bsz, batch, (size_t)max_bindings - n, asks, snap, st)) return -1;
         rc = yklt::device_commit(lp, sequential, bind, fail, handoff);
     }
@@ -288,7 +303,7 @@ int run_d(uint32_t policy, const double* weights,
         const uint64_t c[] = {(uint64_t)hdr[yklt::H_SUBRUNS], (uint64_t)hdr[yklt::H_FULLSCANS], (uint64_t)hdr[yklt::H_SORTS],
                               (uint64_t)hdr[yklt::H_ELEMS], (uint64_t)hdr[yklt::H_QUICK], (uint64_t)hdr[yklt::H_ESC],
                               st.lattice_handoffs, st.batches, attempts, st.uniform_retries, st.uniform_asks, st.uniform_runs,
-                              st.uniform_elements, passes, singles, round_asks, round_stretches, parked};
+                              st.uniform_elements, passes, singles, round_asks, round_stretches, parked, 1};
         std::copy(c, c + sizeof(c) / sizeof(c[0]), stats_out);
     }
     return 0;
@@ -297,7 +312,8 @@ int run_d(uint32_t policy, const double* weights,
 }  // namespace
 
 // same argument list as engine_host_run (tests/host/engine_shim.cpp) so that the Python harness is shared; epoch_limit,
-// speculate and share_rows do not apply.  Returns 100 when the snapshot is not eligible for the device commit.
+// speculate and share_rows do not apply.  Returns INELIGIBLE when the snapshot is not eligible for the forced device
+// commit, HOST_COMMIT when `auto` starts the cycle on the host commit.
 extern "C" int device_host_run(int D, uint32_t policy, const double* weights,
     uint32_t nN, const int64_t* n_total, const int64_t* n_avail, const uint64_t* n_taint, const uint64_t* n_label,
     const uint32_t* n_flags, const uint32_t* n_rank,

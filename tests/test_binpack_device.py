@@ -160,24 +160,37 @@ def test_nan_score_is_a_clean_error(oracle, commit):
         assert e.stats()["lattice_cycles"] == 2
 
 
-def test_counters_equal_the_shim(oracle, dshim):
-    """uniform runs, fills (lattice launches: one per fill, no other kernel runs), uniform asks and hand-offs.  The batch
-    holds every ask: in a placement-insensitive order the engine decides the whole order in one batch, the shim in
-    `batch`-sized ones"""
+def test_counters_equal_the_shim(oracle, dshim, monkeypatch):
+    """uniform runs, fills (lattice launches: one per fill, no other kernel runs), uniform asks and hand-offs, at the default
+    batch.  Forced `device`: in a placement-insensitive order the engine decides the whole order in one batch, the shim in
+    `batch`-sized ones, so the shim's batch holds every ask.  `auto`: the engine and the shim choose the same commit, and
+    count the same where it is the device"""
+    from device_shim import HOST_COMMIT
+    monkeypatch.setenv("YK_UNIFORM_MIN", "64")   # `auto`'s screen, scaled down to these snapshots
+    on_device = 0
     for s in (synth.reference_shape(600, 40, 125, policy=BP), overcommitted(True), mixed_signature_gangs(1),
               synth.runny(synth.perf(300, 10, 60, masks=True, policy=BP), 5), synth.runny(synth.hier(200, 2, 3, 2, 30, policy=BP), 6),
               synth.gangs(300, 60, 5, seed=1, fill=2.0, policy=BP)):
-        batch = 8192
         if s.name.startswith("gangs"):
             s.ask_req[:] = s.ask_req[0]
         want = oracle.run(s)
-        dev = _fill(s, want, batch=batch)
-        c = []
-        rc, ask, node, _, _ = shim_run(dshim, s, stats=c, batch=batch)
-        assert rc == 0 and np.array_equal(ask, want["ask"]) and np.array_equal(node, want["node"])
-        c = c[0]
-        assert (dev["uniform_runs"], dev["uniform_asks"], dev["lattice_handoffs"], dev["lattice_launches"]) == \
-            (c["uniform_runs"], c["uniform_asks"], c["handoffs"], c["uniform_attempts"]), s.name
+        for commit in ("device", "auto"):
+            dev = _run(s, want, commit=commit, binpacking_device=True)
+            c = []
+            if commit == "device":
+                rc, ask, node, _, _ = shim_run(dshim, s, stats=c, batch=max(4096, s.n_asks))
+            else:
+                rc, ask, node, _, _ = shim_run(dshim, s, stats=c, auto=True, uniform=(64, 0), batch=4096)
+                if rc == HOST_COMMIT:
+                    assert dev["lattice_cycles"] == 0, s.name
+                    continue
+                on_device += 1
+            assert rc == 0 and np.array_equal(ask, want["ask"]) and np.array_equal(node, want["node"])
+            c = c[0]
+            assert dev["lattice_cycles"] == 1 and dev["uniform_retries"] == 0 and dev["lattice_subruns"] == 0, (s.name, commit, dev)
+            assert (dev["uniform_runs"], dev["uniform_asks"], dev["lattice_handoffs"], dev["lattice_launches"]) == \
+                (c["uniform_runs"], c["uniform_asks"], c["handoffs"], c["uniform_attempts"]), (s.name, commit)
+    assert on_device > 0
 
 
 # ---- sessions: releases, node upserts, removals, cordons between cycles ----

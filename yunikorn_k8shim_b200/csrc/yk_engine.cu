@@ -46,14 +46,6 @@ namespace {
 constexpr int NPT = YK_NPT;       // sorted-node positions per sweep thread
 constexpr int AC = 128;           // asks per sweep CTA chunk
 constexpr int NODE_TILE = YK_SWEEP_THREADS * NPT;
-// round commit (yk_rounds.h), measured on H100 by scripts/round_prof.py (DESIGN.md §6.3): mask-free fair cycles of 10 000
-// asks and more are faster on it, 5 000 are not
-constexpr int RD_MIN = 10000;               // fewest pending asks for which a mask-free cycle starts on the device commit
-constexpr double RD_US_PER_ASK = 0.16;      // whole cycle per ask on the round commit (config 2: 7.4-8.2 ms / 50 000)
-constexpr double RD_HOST_US_PER_ASK = 0.28; // ... and on the sweep + host commit (config 2: 12.4-19.7 ms / 50 000)
-// binpacking fill (yk_uniform.h, YK_FLAG_BINPACKING_DEVICE), measured on H100 by scripts/binpack_prof.py (DESIGN.md §6.4)
-constexpr double BP_FILL_US = 140.0;        // whole cycle per fill (runny config 2: 737 ms / 5 198 fills), whatever the run's length
-constexpr double BP_HOST_US_PER_ASK = 0.1;  // whole cycle per ask on the sweep + host commit (0.106-0.137 us on the three shapes)
 
 inline size_t round_up(size_t v, size_t m) { return (v + m - 1) / m * m; }
 
@@ -264,7 +256,6 @@ struct yk_engine {
     std::vector<uint32_t> ep_reps;
     Dev<uint32_t> ep_d_batch, ep_d_fit; Pin<uint32_t> ep_h_batch, ep_h_fit;
     cudaEvent_t ep_ev = nullptr, ep_s0 = nullptr, ep_s1 = nullptr;
-    uint32_t n_shapes = 0, n_sigs = 0;
     SigTable sigs; std::vector<uint32_t> ep_local, ep_seen; uint32_t ep_stamp = 0;
     // device-resident ordered commit (yk_lattice.h): node records, ping-pong node order, per-batch staging
     bool lt_allowed = true;                  // !YK_FLAG_HOST_COMMIT, single GPU
@@ -284,10 +275,7 @@ struct yk_engine {
     cudaEvent_t ev_l0 = nullptr, ev_l1 = nullptr;
     // uniform runs (yk_uniform.h): allocated on first use; element buffers hold UN_EMAX generated elements
     bool hp_on = false; double hp[8] = {0, 0, 0, 0, 0, 0, 0, 0}; uint64_t hp_n = 0;
-    bool un_hint = false;                       // this cycle's pending asks look like long uniform runs (auto commit: size the first batch for it)
-    bool lt_plan_ready = false;                 // h_lt_meta/shp/sig and un_segs already describe slot[0]'s batch (built by the commit choice)
     bool un_alloc = false, un_ord_stale = false;   // un_ord_stale: uniform runs moved nodes since d_ord was last written
-    const uint32_t* lt_shape_ids = nullptr;     // per ask: a number equal for equal request vectors (a_shape, or a_sigid: finer, still exact)
     int un_min = 2048;                          // shortest run that takes the uniform path (YK_UNIFORM_MIN)
     int un_depth = 0;                           // first depth of a uniform run's attempt (YK_UNIFORM_DEPTH); 0: ykun::first_depth
     Dev<unsigned long long> d_un_ekey[2], d_un_bk, d_un_rkey[2], d_un_rrn[2];
@@ -296,11 +284,10 @@ struct yk_engine {
     Dev<uint8_t> d_un_cub; size_t un_cub_bytes = 0;
     std::vector<ykun::Segment> un_segs;
     // round commit (yk_rounds.h) of mask-free stretches, automatic commit only
-    int rd_min = RD_MIN;                        // fewest pending asks for which a mask-free cycle starts on it (YK_ROUND_MIN; 0: never)
+    int rd_min = yklt::RD_MIN;                  // fewest pending asks for which a mask-free cycle starts on it (YK_ROUND_MIN; 0: never)
     int rd_window = ykrd::WCAP;                 // candidates per round (YK_ROUND_WINDOW: a testing knob)
     int rd_guard = ykrd::GUARD;                  // asks per pass below which a stretch hands over to the host commit (YK_ROUND_GUARD)
     uint64_t rd_taints = 0;                     // this cycle: union of the live nodes' taints
-    bool rd_maskfree = false;                   // this cycle: every pending ask is round-eligible (no gang, no masks)
     size_t rd_smem = 0;
     Dev<yklt::Ent> d_rd_spent; Dev<int> d_rd_hdr; Pin<int> h_rd_hdr;
     Dev<int64_t> d_rd_req;                      // [maxA][D]: a stretch's requests in stretch order (ykrd::Args::sreq)
@@ -1639,23 +1626,15 @@ void bind_one(yk_engine* e, Cycle& c, uint32_t a, uint32_t node) {
     ++c.n;
 }
 
-// fill one batch; YK_ERR_ARG when a gang cannot fit any batch
-int fill_batch(yk_engine* e, size_t& bsz, size_t bmax, size_t cap_user, Slot& sl, yk_stats_t& st) {
-    sl.B = 0; sl.nchunks = 0;
-    if (!yk::fill_batch(e->ord, bsz, bmax, cap_user, sl.asks, sl.snap, st))
-        return e->fail(YK_ERR_ARG, yk::GANG_TOO_BIG);
-    return YK_OK;
-}
-
-// The cycle on the device commit.  slot[0] already holds the first batch.  Returns with handoff = true when the rest of
-// the cycle belongs to the host commit.
-int run_lattice(yk_engine* e, Cycle& c, bool& handoff) {
+// The cycle on the device commit.  slot[0] already holds the first batch (yklt::choose_commit).  Returns with handoff =
+// true when the rest of the cycle belongs to the host commit.
+int run_lattice(yk_engine* e, Cycle& c, yklt::Choice& ch, bool& handoff) {
     handoff = false;
     int rc = lt_prepare(e);
     if (rc) return rc;
     Slot& A = e->slot[0];
-    yklt::Loop lp{e->ord, e->cm.t, e->lt_shape_ids, e->a_sigid.data(), A.asks, A.snap, c.result,
-                  e->h_lt_meta.p, e->h_lt_shp.p, e->h_lt_sig.p, e->un_segs, e->lt_plan_ready,
+    yklt::Loop lp{e->ord, e->cm.t, ch.shape_ids, e->a_sigid.data(), A.asks, A.snap, c.result,
+                  e->h_lt_meta.p, e->h_lt_shp.p, e->h_lt_sig.p, e->un_segs, ch.plan_ready,
                   yklt::min_run(e->cfg.policy == YK_POLICY_BINPACKING, e->un_min), e->nlive == 0,
                   e->ord.insensitive ? (size_t)e->maxA : (size_t)e->batch, c.max_bindings, c.n, e->st};
     if (e->nlive && !A.asks.empty()) {   // the initial order's NaN flag (device_order) is checked before the first batch
@@ -1733,18 +1712,13 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
     const bool dev_policy = e->cfg.policy == YK_POLICY_FAIR || (bp && e->bp_device);
     const bool force_lattice = e->lt_allowed && e->lt_force && dev_policy;
     const bool auto_lattice = e->lt_allowed && !e->lt_force && e->lt_auto && e->un_min > 0 && dev_policy;
+    yklt::Scan scan;   // the pending scan's hints for the commit choice
     e->worker.submit([&] {
         const double t_b = now_ms();
         pending.clear();
         pending.reserve(e->a_hi);
         bool any_gang = false;
-        // (longest run of one signature id among consecutive pending asks, in index order: the hint for the automatic commit choice)
-        size_t sig_run = 0, sig_longest = 0;
-        uint32_t sig_prev = YK_NONE;
-        // (and whether every pending ask is free of masks -- yklt::round_eligible -- for the round commit)
-        uint64_t taints = 0;
-        if (auto_lattice) for (uint32_t n = 0; n < e->n_hi; ++n) if (e->n_present[n]) taints |= e->n_taint[n];
-        bool maskfree = auto_lattice && !bp;
+        if (auto_lattice) for (uint32_t n = 0; n < e->n_hi; ++n) if (e->n_present[n]) scan.taints |= e->n_taint[n];
         for (uint32_t a = 0; a < e->a_hi; ++a) {
             uint8_t& st = e->a_state[a];
             if (st == yk::ST_ABSENT || st == yk::ST_ALLOCATED) continue;
@@ -1752,16 +1726,10 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
             if (!e->p_present[e->a_app[a]]) continue;
             pending.push_back(a);
             any_gang = any_gang || e->a_gang[a] != YK_NONE;
-            if (auto_lattice) {
-                const uint32_t g = e->a_sigid[a];
-                if (g == sig_prev) ++sig_run; else { sig_longest = std::max(sig_longest, sig_run); sig_run = 1; sig_prev = g; }
-                maskfree = maskfree && e->a_need[a] == 0 && e->a_deny[a] == 0 && e->a_node[a] == YK_NONE && (taints & ~e->a_tol[a]) == 0;
-            }
+            if (auto_lattice) scan.add(e->cm.t, e->a_sigid.data(), a);
         }
-        sig_longest = std::max(sig_longest, sig_run);
         e->cycle_has_gang = any_gang;
-        e->rd_taints = taints;
-        e->rd_maskfree = maskfree && !any_gang;
+        e->rd_taints = scan.taints;
         if (any_gang) {   // a gang that no batch can hold is an argument error: found before anything is committed
             std::unordered_map<uint64_t, uint32_t> members;
             for (uint32_t a : pending)
@@ -1794,19 +1762,10 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
                     if (++ns > yk_engine::EP_MAX) break;
                 }
             }
-            e->n_sigs = ns;
             e->ep_rows = ns > 0 && ns <= yk_engine::EP_MAX && (uint64_t)ns * 8 <= pending.size();
             e->ep_n = ns;
         }
-        // a hint only (it sizes the first batch, never decides): asks are usually upserted application by application, so a long
-        // run of one signature in index order promises one in the orderer's order
-        e->un_hint = !gang_too_big && auto_lattice &&
-                     ((pending.size() >= (size_t)e->un_min && sig_longest >= (size_t)e->un_min) ||
-                      (e->rd_maskfree && e->rd_min > 0 && pending.size() >= (size_t)e->rd_min));
-        if (!gang_too_big && force_lattice) {   // request-vector numbers for the lattice kernel's windows
-            yklt::assign_shapes(e->cm.t, pending, e->a_shape, &e->n_shapes);
-            e->lt_shape_ids = e->a_shape.data();
-        }
+        if (!gang_too_big) scan.done(e->cm.t, pending, force_lattice, e->a_shape);
         e->ep_uploaded = false; e->ep_landed = true;
         begin_ms = now_ms() - t_b;
     });
@@ -1826,83 +1785,24 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
 
     Cycle c;
     c.max_bindings = max_bindings; c.out = out;
-    // the first batch decides which commit the cycle starts on
-    const bool ins = e->ord.insensitive;
-    bool lattice = false;
-    size_t bsz0 = e->batch;
-    if (force_lattice) {
-        const yklt::Eligibility el = yklt::eligible(e->cm.t, e->n_hi, e->n_present.data(), e->n_total.p, e->maxN, e->n_rank.data(), pending, &e->ranks_unique, &e->cycle_has_gang, e->bp_device);
-        lattice = el.ok;
-        if (lattice && ins) bsz0 = e->maxA;   // the whole static order in one launch
-    }
-    if (auto_lattice && e->un_hint && ins) bsz0 = e->maxA;
-    e->lt_plan_ready = false;
-    rc = fill_batch(e, bsz0, std::max<size_t>(bsz0, e->batch), max_bindings, e->slot[0], e->st);
-    // a big mask-free cycle in a placement-insensitive order: its stretches between uniform runs go to the round commit
-    const bool round_screen = ins && e->rd_maskfree && e->rd_min > 0 && pending.size() >= (size_t)e->rd_min;
-    if (!rc && auto_lattice && ((pending.size() >= (size_t)e->un_min && e->slot[0].asks.size() >= (size_t)e->un_min) || round_screen)) {
-        // Automatic: the device commit decides a uniform run (one request vector, one predicate signature) by a grid-wide sort,
-        // a mask-free stretch by rounds at the front of the node order (DESIGN.md §6.3), everything else through a
-        // sequential chain that one host core still does faster (DESIGN.md §6.2).  So the cycle starts on the device when
-        // its order is made of long uniform runs or when it is big and mask-free.  Cheap screens first -- the longest run
-        // of one signature id in the first batch, the pending scan's mask-free flag -- and only then the eligibility test.
-        const std::vector<uint32_t>& as = e->slot[0].asks;
-        size_t longest = 0, run = 1;
-        for (size_t i = 1; i <= as.size(); ++i) {
-            if (i < as.size() && e->a_sigid[as[i]] == e->a_sigid[as[i - 1]]) { ++run; continue; }
-            longest = std::max(longest, run);
-            run = 1;
-        }
-        if (longest >= (size_t)e->un_min || round_screen) {
-            const yklt::Eligibility el = yklt::eligible(e->cm.t, e->n_hi, e->n_present.data(), e->n_total.p, e->maxN, e->n_rank.data(), pending, &e->ranks_unique, &e->cycle_has_gang, e->bp_device);
-            if (el.ok) {
-                // signature ids double as shape numbers: equal signatures request equal vectors; two signatures with one request
-                // only make the (rare, here) windowed stretches see one more shape
-                e->lt_shape_ids = e->a_sigid.data();
-                if (ins && e->slot[0].asks.size() < pending.size() && bsz0 < (size_t)e->maxA) {   // the whole static order in one batch
-                    e->ord.unfill(e->slot[0].snap, e->slot[0].asks, 0);
-                    size_t b = e->maxA;
-                    rc = fill_batch(e, b, e->maxA, max_bindings, e->slot[0], e->st);
-                }
-                if (!rc) {
-                    const size_t B0 = e->slot[0].asks.size();
-                    yklt::build_meta(e->cm.t, e->lt_shape_ids, e->a_sigid.data(), e->slot[0].asks, e->h_lt_meta.p, e->h_lt_shp.p, e->h_lt_sig.p);
-                    ykun::plan_segments(e->h_lt_meta.p, e->h_lt_shp.p, e->h_lt_sig.p, (int)B0, yklt::min_run(bp, e->un_min), e->un_segs);
-                    // measured costs (H100, bench.py device_commit / host_commit arms): a uniform run ~0.2-0.3 ms whatever its
-                    // length (16 launches, one round trip), a windowed ask ~0.35 us, an ask on the host commit ~0.08-0.13 us
-                    // (the host side gets a 30 % margin); a round stretch is priced in whole-cycle time per ask on both sides
-                    // (scripts/round_prof.py), which is how it was measured
-                    double dev_us = 0, host_us = 0;
-                    // binpacking: a fill per run at its fixed cost; a stretch hands the rest of the cycle to the host commit
-                    if (bp) for (const ykun::Segment& sg : e->un_segs) {
-                        dev_us += sg.uniform ? BP_FILL_US : BP_HOST_US_PER_ASK * sg.len;
-                        host_us += BP_HOST_US_PER_ASK * sg.len;
-                    }
-                    else for (const ykun::Segment& sg : e->un_segs) {
-                        const bool rounds = !sg.uniform && yklt::round_eligible(e->cm.t, ins, e->rd_taints, e->slot[0].asks.data() + sg.off, (size_t)sg.len);
-                        dev_us += sg.uniform ? 250.0 : (rounds ? RD_US_PER_ASK : 0.35) * sg.len;
-                        host_us += (rounds ? RD_HOST_US_PER_ASK : 0.7 * 0.08) * sg.len;
-                    }
-                    lattice = dev_us < host_us;
-                    e->lt_plan_ready = lattice;
-                }
-            }
-        }
-    }
-    if (!rc && !lattice && e->slot[0].asks.size() > e->batch) {   // the first fill was sized for the device commit
-        e->ord.unfill(e->slot[0].snap, e->slot[0].asks, 0);
-        size_t b = e->batch;
-        rc = fill_batch(e, b, e->batch, max_bindings, e->slot[0], e->st);
-    }
+    // which commit the cycle starts on, and its first batch (a hand-off refills the slot, still unlaunched)
+    Slot& first = e->slot[0];
+    first.B = 0; first.nchunks = 0;
+    const yklt::ChoiceIn in{e->ord, e->cm.t, pending, e->n_hi, e->n_present.data(), e->n_total.p, e->maxN, e->n_rank.data(),
+                            &e->ranks_unique, &e->cycle_has_gang, force_lattice, auto_lattice, e->bp_device, e->un_min, e->rd_min,
+                            scan, e->batch, e->maxA, max_bindings, e->a_shape.data(), e->a_sigid.data(), first.asks, first.snap,
+                            e->h_lt_meta.p, e->h_lt_shp.p, e->h_lt_sig.p, e->un_segs, e->st};
+    yklt::Choice choice;
+    if (!yklt::choose_commit(in, choice)) rc = e->fail(YK_ERR_ARG, yk::GANG_TOO_BIG);
     e->lt_active = false;
     hp(3);
     if (!rc) {
-        if (lattice) {
+        if (choice.device) {
             e->lt_active = true;
             e->order_enqueued = false;   // consumed by lt_prepare; a hand-over sorts again from the exported tables
             e->st.lattice_cycles++;
             bool handoff = false;
-            rc = run_lattice(e, c, handoff);
+            rc = run_lattice(e, c, choice, handoff);
             if (!rc) {
                 const int rce = lt_export(e);   // node tables current again, host and device
                 e->lt_active = false;
@@ -1917,8 +1817,8 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
             }
             if (!rc && handoff && c.n < max_bindings) {
                 size_t b = e->batch;
-                rc = fill_batch(e, b, e->batch, (size_t)max_bindings - c.n, e->slot[0], e->st);
-                if (!rc) rc = run_host(e, c);
+                rc = yk::fill_batch(e->ord, b, e->batch, (size_t)max_bindings - c.n, first.asks, first.snap, e->st)
+                         ? run_host(e, c) : e->fail(YK_ERR_ARG, yk::GANG_TOO_BIG);
             }
         } else {
             rc = run_host(e, c);

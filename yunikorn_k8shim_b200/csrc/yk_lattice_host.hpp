@@ -1,8 +1,9 @@
 // yk_lattice_host.hpp -- the cycle's two batch loops and the host side of the device commit (yk_lattice.h, yk_uniform.h).
 // yk::host_commit is the host commit's loop (speculation, settle and rewind, batch sizing, epoch ends); yklt::device_commit
 // is the device commit's, around the per-entry meta words the kernel reads, the test that decides whether a cycle may use
-// the device commit at all, the segment loop and a uniform run's attempts.  Both share fill_batch, settle, the batch-size
-// rule and the no-node rule.  No CUDA in here: csrc/yk_engine.cu runs both loops with the sweep and the kernels,
+// the device commit at all, the segment loop and a uniform run's attempts.  yklt::choose_commit decides which of the two a
+// cycle starts on and fills its first batch.  Both loops share fill_batch, settle, the batch-size rule and the no-node
+// rule.  No CUDA in here: csrc/yk_engine.cu runs both loops with the sweep and the kernels,
 // tests/host/engine_shim.cpp runs the host loop with a CPU sweep and tests/host/device_shim.cpp the device loop with the
 // kernels' per-item code.
 #pragma once
@@ -233,7 +234,7 @@ inline bool same_request(const yk::CommitTables& t, uint32_t a, uint32_t b) {
 }
 
 // Dense numbers for the distinct request vectors ("shapes") of the cycle's pending asks: a_shape[ask].  Equal numbers <=>
-// equal vectors (hash table, equality always confirmed on the full vector).
+// equal vectors (hash table, equality always confirmed on the full vector); *n_shapes = how many, unless n_shapes is null.
 inline void assign_shapes(const yk::CommitTables& t, const std::vector<uint32_t>& pending, std::vector<uint32_t>& a_shape, uint32_t* n_shapes) {
     struct Slot { uint32_t ask; uint32_t id; };
     size_t cap = 64;
@@ -251,7 +252,7 @@ inline void assign_shapes(const yk::CommitTables& t, const std::vector<uint32_t>
             x = (x + 1) & (cap - 1);
         }
     }
-    *n_shapes = ns;
+    if (n_shapes) *n_shapes = ns;
 }
 
 // Dense numbers for the distinct predicate signatures of the given asks (the engine keeps these up to date as asks are
@@ -288,30 +289,6 @@ inline void build_meta(const yk::CommitTables& t, const uint32_t* a_shape, const
         }
         meta[i] = m; shp[i] = a_shape[a]; sig[i] = a_sigid[a];
     }
-}
-
-// How many sub-run windows the kernel's staging rules (at most SMAX shapes, SIGCAP signatures, KCAP asks) cut the batch
-// into at least: the engine only starts a cycle on the device commit when the windows are long enough to pay for a sub-run.
-inline size_t estimate_windows(const uint32_t* shp, const uint32_t* sig, size_t B) {
-    size_t windows = 0, i = 0;
-    std::vector<uint32_t> seen(512, 0xFFFFFFFFu);
-    while (i < B) {
-        uint32_t shapes[SMAX];
-        int ns = 0, rows = 0;
-        std::fill(seen.begin(), seen.end(), 0xFFFFFFFFu);
-        size_t j = i;
-        for (; j < B && j - i < (size_t)KCAP; ++j) {
-            int k = 0;
-            while (k < ns && shapes[k] != shp[j]) ++k;
-            if (k == ns) { if (ns == SMAX) break; shapes[ns++] = shp[j]; }
-            size_t x = (sig[j] * 2654435761u) >> 23;   // 9 bits
-            while (seen[x] != 0xFFFFFFFFu && seen[x] != sig[j]) x = (x + 1) & 511;
-            if (seen[x] == 0xFFFFFFFFu) { if (rows == SIGCAP) break; seen[x] = sig[j]; ++rows; }
-        }
-        ++windows;
-        i = j > i ? j : i + 1;
-    }
-    return windows;
 }
 
 // What the lattice commit relies on (DESIGN.md "lattice commit"):
@@ -427,6 +404,127 @@ inline auto route_stretches(bool rounds_on, const yk::CommitTables& t, bool inse
 
 // The shortest uniform run of a cycle on the device commit (0: none): under binpacking every maximal run is one fill.
 inline int min_run(bool binpacking, int un_min) { return binpacking ? 1 : un_min; }
+
+// round commit (yk_rounds.h), measured on H100 by scripts/round_prof.py (DESIGN.md §6.3): mask-free fair cycles of 10 000
+// asks and more are faster on it, 5 000 are not
+constexpr int RD_MIN = 10000;               // fewest pending asks for which a mask-free cycle starts on the device commit
+constexpr double RD_US_PER_ASK = 0.16;      // whole cycle per ask on the round commit (config 2: 7.4-8.2 ms / 50 000)
+constexpr double RD_HOST_US_PER_ASK = 0.28; // ... and on the sweep + host commit (config 2: 12.4-19.7 ms / 50 000)
+// binpacking fill (yk_uniform.h, YK_FLAG_BINPACKING_DEVICE), measured on H100 by scripts/binpack_prof.py (DESIGN.md §6.4)
+constexpr double BP_FILL_US = 140.0;        // whole cycle per fill (runny config 2: 737 ms / 5 198 fills), whatever the run's length
+constexpr double BP_HOST_US_PER_ASK = 0.1;  // whole cycle per ask on the sweep + host commit (0.106-0.137 us on the three shapes)
+
+// The pending scan's part of the commit choice: the caller lists the cycle's pending asks in index order, passes each to
+// add() under `auto` (the engine does so on its helper thread, next to its own bookkeeping), then calls done() once.
+struct Scan {
+    uint64_t taints = 0;         // union of the live nodes' taints
+    bool maskfree = true;        // every pending ask is round-eligible (round_eligible: no gang, no masks)
+    // the longest run of one signature id in index order: asks are usually upserted application by application, so a long
+    // run in index order promises one in the orderer's order
+    size_t longest = 0, run = 0;
+    uint32_t prev = yk::CNONE;
+    void add(const yk::CommitTables& t, const uint32_t* a_sigid, uint32_t a) {
+        run = a_sigid[a] == prev ? run + 1 : 1; prev = a_sigid[a]; longest = std::max(longest, run);
+        maskfree = maskfree && t.a_gang[a] == yk::CNONE && t.a_need[a] == 0 && t.a_deny[a] == 0 && t.a_node[a] == yk::CNONE &&
+                   (taints & ~t.a_tol[a]) == 0;
+    }
+    // forced: number the request vectors, the shapes of the lattice kernel's windows
+    void done(const yk::CommitTables& t, const std::vector<uint32_t>& pending, bool forced, std::vector<uint32_t>& a_shape) {
+        if (forced) assign_shapes(t, pending, a_shape, nullptr);
+    }
+};
+
+// What the commit choice reads and fills; the caller owns all of it.
+struct ChoiceIn {
+    yk::Orderer& ord;                     // the cycle begun on `pending`
+    const yk::CommitTables& ct;
+    const std::vector<uint32_t>& pending;
+    uint32_t n_hi; const uint8_t* n_present; const int64_t* n_total; size_t ldn; const uint32_t* n_rank;   // eligible's nodes
+    const bool* ranks_unique; const bool* any_gang;                                                         // ... and its caches
+    bool forced, automatic, binpacking_ok;   // YK_FLAG_DEVICE_COMMIT (every eligible cycle), `auto` (the cost rule), YK_FLAG_BINPACKING_DEVICE
+    int un_min, rd_min;                   // shortest uniform run, fewest pending asks for the round commit (0: never)
+    const Scan& scan;
+    size_t batch, maxA;                   // the largest batch, the whole static order
+    uint32_t max_bindings;
+    const uint32_t* a_shape; const uint32_t* a_sigid;   // Scan::done's request-vector numbers (forced), signature ids
+    std::vector<uint32_t>& asks; yk::Orderer::Snap& snap;   // the first batch
+    uint32_t* meta; uint32_t* shp; uint32_t* sig; std::vector<ykun::Segment>& segs;   // its plan (build_meta, plan_segments)
+    yk_stats_t& st;
+};
+
+struct Choice {
+    bool device = false;                  // the cycle starts on the device commit, else on the host commit
+    const uint32_t* shape_ids = nullptr;  // build_meta's shape numbers: a_shape when forced, the signature ids under auto
+    bool plan_ready = false;              // meta, shp, sig and segs already describe the first batch
+};
+
+// Which commit the cycle starts on, and its first batch (filled into in.asks, not launched).  Forced: the device commit
+// when the cycle is eligible, the whole static order in one launch when the order is placement-insensitive.  Automatic:
+// the device commit decides a uniform run (one request vector, one predicate signature) by a grid-wide sort, a mask-free
+// stretch by rounds at the front of the node order (DESIGN.md §6.3), everything else through a sequential chain that one
+// host core still does faster (DESIGN.md §6.2).  So the cycle starts on the device when its order is made of long uniform
+// runs or when it is big and mask-free.  Cheap screens first -- the pending scan's hints, the longest run of one signature
+// id in the first batch -- then the eligibility test, then the cost rule on the first batch's plan.  False when a gang
+// fits no batch.
+inline bool choose_commit(const ChoiceIn& in, Choice& out) {
+    out = Choice{};
+    const bool ins = in.ord.insensitive, bp = in.ct.policy == YK_POLICY_BINPACKING;
+    const size_t np = in.pending.size();
+    auto is_eligible = [&] {
+        return eligible(in.ct, in.n_hi, in.n_present, in.n_total, in.ldn, in.n_rank, in.pending, in.ranks_unique, in.any_gang,
+                        in.binpacking_ok).ok;
+    };
+    auto refill = [&](size_t b) {   // undo the first fill, fill again at b
+        in.ord.unfill(in.snap, in.asks, 0);
+        return yk::fill_batch(in.ord, b, b, in.max_bindings, in.asks, in.snap, in.st);
+    };
+    size_t bsz = in.batch;
+    if (in.forced) {
+        out.device = is_eligible();
+        out.shape_ids = in.a_shape;
+        if (out.device && ins) bsz = in.maxA;   // the whole static order in one launch
+    }
+    // a big mask-free cycle in a placement-insensitive order: its stretches between uniform runs go to the round commit
+    const bool maskfree_big = in.automatic && !bp && in.scan.maskfree && in.rd_min > 0 && np >= (size_t)in.rd_min;
+    const bool round_screen = ins && maskfree_big;
+    // the hints only size the first batch, they never decide
+    if (in.automatic && ins && ((np >= (size_t)in.un_min && in.scan.longest >= (size_t)in.un_min) || maskfree_big)) bsz = in.maxA;
+    if (!yk::fill_batch(in.ord, bsz, std::max(bsz, in.batch), in.max_bindings, in.asks, in.snap, in.st)) return false;
+    if (in.automatic && ((np >= (size_t)in.un_min && in.asks.size() >= (size_t)in.un_min) || round_screen)) {
+        size_t longest = 0, run = 1;
+        for (size_t i = 1; i <= in.asks.size(); ++i) {
+            if (i < in.asks.size() && in.a_sigid[in.asks[i]] == in.a_sigid[in.asks[i - 1]]) { ++run; continue; }
+            longest = std::max(longest, run);
+            run = 1;
+        }
+        if ((longest >= (size_t)in.un_min || round_screen) && is_eligible()) {
+            // signature ids double as shape numbers: equal signatures request equal vectors; two signatures with one request
+            // only make the (rare, here) windowed stretches see one more shape
+            out.shape_ids = in.a_sigid;
+            if (ins && in.asks.size() < np && bsz < in.maxA && !refill(in.maxA)) return false;   // the whole static order in one batch
+            build_meta(in.ct, out.shape_ids, in.a_sigid, in.asks, in.meta, in.shp, in.sig);
+            ykun::plan_segments(in.meta, in.shp, in.sig, (int)in.asks.size(), min_run(bp, in.un_min), in.segs);
+            // measured costs (H100, bench.py device_commit / host_commit arms): a uniform run ~0.2-0.3 ms whatever its
+            // length (16 launches, one round trip), a windowed ask ~0.35 us, an ask on the host commit ~0.08-0.13 us (the
+            // host side gets a 30 % margin); a round stretch is priced in whole-cycle time per ask on both sides
+            // (scripts/round_prof.py), which is how it was measured; under binpacking a fill per run at its fixed cost, and
+            // a stretch hands the rest of the cycle to the host commit
+            double dev_us = 0, host_us = 0;
+            if (bp) for (const ykun::Segment& sg : in.segs) {
+                dev_us += sg.uniform ? BP_FILL_US : BP_HOST_US_PER_ASK * sg.len;
+                host_us += BP_HOST_US_PER_ASK * sg.len;
+            }
+            else for (const ykun::Segment& sg : in.segs) {
+                const bool rounds = !sg.uniform && round_eligible(in.ct, ins, in.scan.taints, in.asks.data() + sg.off, (size_t)sg.len);
+                dev_us += sg.uniform ? 250.0 : (rounds ? RD_US_PER_ASK : 0.35) * sg.len;
+                host_us += (rounds ? RD_HOST_US_PER_ASK : 0.7 * 0.08) * sg.len;
+            }
+            out.device = out.plan_ready = dev_us < host_us;
+        }
+    }
+    // the first fill was sized for the device commit
+    return out.device || in.asks.size() <= in.batch || refill(in.batch);
+}
 
 // One planned batch of a cycle on the device commit (run_segments over the asks `asks`): under binpacking the stretches
 // between the uniform runs go to the host commit (hand_off), otherwise through route_stretches.

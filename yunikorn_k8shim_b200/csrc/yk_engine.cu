@@ -63,14 +63,16 @@ struct Dev {
 template <typename T>
 struct Pin {
     T* p = nullptr; size_t n = 0;
-    cudaError_t alloc(size_t count) {
+    T* d = nullptr;   // alloc(count, true): the device's address of the same memory (mapped), which kernels write directly
+    cudaError_t alloc(size_t count, bool mapped = false) {
         free();
         n = count;
-        cudaError_t e = cudaMallocHost((void**)&p, std::max<size_t>(count, 1) * sizeof(T));
+        cudaError_t e = cudaHostAlloc((void**)&p, std::max<size_t>(count, 1) * sizeof(T), mapped ? cudaHostAllocMapped : cudaHostAllocDefault);
         if (e == cudaSuccess) memset(p, 0, std::max<size_t>(count, 1) * sizeof(T));
+        if (e == cudaSuccess && mapped) e = cudaHostGetDevicePointer((void**)&d, p, 0);
         return e;
     }
-    void free() { if (p) cudaFreeHost(p); p = nullptr; n = 0; }
+    void free() { if (p) cudaFreeHost(p); p = nullptr; d = nullptr; n = 0; }
     T& operator[](size_t i) { return p[i]; }
     const T& operator[](size_t i) const { return p[i]; }
     ~Pin() { free(); }
@@ -290,6 +292,9 @@ struct yk_engine {
     uint64_t rd_taints = 0;                     // this cycle: union of the live nodes' taints
     size_t rd_smem = 0;
     Dev<yklt::Ent> d_rd_spent; Dev<int> d_rd_hdr; Pin<int> h_rd_hdr;
+    // mapped: the round kernel's results (indexed like the staged batch) and its decided count (ykrd::Args::prog), which the
+    // host reads while the kernel runs
+    Pin<uint32_t> h_rd_res; Pin<int> h_rd_prog;
     Dev<int64_t> d_rd_req;                      // [maxA][D]: a stretch's requests in stretch order (ykrd::Args::sreq)
     Dev<uint32_t> pre_q; Dev<int64_t> pre_v; Dev<int32_t> pre_o;   // yk_preemption_search staging, grown on demand
     // yk_filter_nodes: its own node order (so a cycle's sort buffers are never touched) and per-chunk buffers, grown on demand
@@ -698,8 +703,11 @@ int lt_window(yk_engine* e, size_t off, size_t B) {
     return YK_OK;
 }
 
-// One round-eligible stretch [off, off + B) of the staged batch through yk_rounds_kernel.
-int lt_rounds(yk_engine* e, size_t off, size_t B, int* status, size_t* consumed) {
+// One round-eligible stretch [off, off + B) of the staged batch through yk_rounds_kernel.  Its results land in the mapped
+// h_rd_res at the same offset; while the kernel runs, ahead(off, to) is called for every newly published decided prefix
+// [off, to), which the caller settles behind the kernel (yklt::settle_ahead).
+template <class Ahead>
+int lt_rounds(yk_engine* e, size_t off, size_t B, int* status, size_t* consumed, Ahead&& ahead) {
     cudaStream_t s = e->stream;
     { const int rco = un_reorder(e); if (rco) return rco; }
     ykrd::Args a{};
@@ -708,14 +716,29 @@ int lt_rounds(yk_engine* e, size_t off, size_t B, int* status, size_t* consumed)
     a.rec = e->d_rec.p; a.RS = e->lt_RS; a.ord[0] = e->d_ord[0].p; a.ord[1] = e->d_ord[1].p; a.cur = e->d_lt_cur.p;
     a.nlive = (int)e->nlive; a.spent = e->d_rd_spent.p;
     a.a_req = e->d_areq.p; a.lda = e->maxA; a.a_tol = e->d_atol.p; a.a_need = e->d_aneed.p; a.a_deny = e->d_adeny.p; a.a_node = e->d_anode.p;
-    a.asks = e->d_lt_asks.p + off; a.B = (int)B; a.sreq = e->d_rd_req.p; a.res = e->d_lt_res.p + off; a.hdr = e->d_rd_hdr.p;
+    a.asks = e->d_lt_asks.p + off; a.B = (int)B; a.sreq = e->d_rd_req.p; a.res = e->h_rd_res.d + off; a.hdr = e->d_rd_hdr.p;
+    a.prog = e->h_rd_prog.d;
     a.window = std::max(1, std::min(e->rd_window, ykrd::WCAP)); a.guard = e->rd_guard;
     a.prof = e->lt_prof ? e->d_lt_prof.p + 16 : nullptr;
+    __atomic_store_n(e->h_rd_prog.p, 0, __ATOMIC_RELAXED);   // (no kernel that writes it is in flight)
     CK(cudaEventRecord(e->ev_l0, s));
     launch_rounds(e->D, a, e->rd_smem, s);
     CK(cudaGetLastError());
     CK(cudaEventRecord(e->ev_l1, s));
     CK(cudaMemcpyAsync(e->h_rd_hdr.p, e->d_rd_hdr.p, ykrd::R_WORDS * sizeof(int), cudaMemcpyDeviceToHost, s));
+    // settle behind the kernel until it ends; the count is read after the query, so the last pass sees its final value.  The
+    // kernel never waits for the host: this loop only reads.
+    for (size_t seen = 0;;) {
+        const bool ended = cudaEventQuery(e->ev_l1) != cudaErrorNotReady;
+        const size_t t = (size_t)__atomic_load_n(e->h_rd_prog.p, __ATOMIC_ACQUIRE);
+        if (t > seen && t <= B) {
+            const double t0 = e->hp_on ? now_ms() : 0;
+            ahead(off, off + t);
+            seen = t;
+            if (e->hp_on) e->hp[7] += now_ms() - t0;   // YK_PROFILE_HOST: settle time hidden behind the kernel
+        }
+        if (ended) break;
+    }
     CK(cudaStreamSynchronize(s));
     float ms = 0;
     cudaEventElapsedTime(&ms, e->ev_l0, e->ev_l1);
@@ -726,19 +749,28 @@ int lt_rounds(yk_engine* e, size_t off, size_t B, int* status, size_t* consumed)
     *status = h[ykrd::R_STATUS];
     *consumed = (size_t)h[ykrd::R_CONSUMED];
     if (*consumed > B) return e->fail(YK_ERR_CUDA, "round kernel returned a bad header");
+    e->st.d2h_bytes += 4 * *consumed;   // the results, written straight into host memory
     e->st.round_passes += (uint64_t)h[ykrd::R_PASSES]; e->st.round_single_steps += (uint64_t)h[ykrd::R_SINGLES];
     e->st.round_asks += *consumed;
     return YK_OK;
 }
 
 // One batch of slot[0] (segments planned in e->un_segs) through yklt::run_segments; the decided entries' nodes land in
-// `result`.  Blocks until it is decided.
-int lt_batch(yk_engine* e, size_t B, int* status, size_t* done, std::vector<uint32_t>& result) {
+// `result`.  Blocks until it is decided; ahead(res, off, to) settles entries of a round stretch while its kernel runs (res:
+// the batch's results as the round kernel writes them).
+template <class Ahead>
+int lt_batch(yk_engine* e, size_t B, int* status, size_t* done, std::vector<uint32_t>& result, Ahead&& ahead) {
     cudaStream_t s = e->stream;
     memcpy(e->h_lt_asks.p, e->slot[0].asks.data(), 4 * B);
     bool staged = false, asks_staged = false;   // only the windowed kernel reads the per-entry words, the round kernel the asks
-    auto uniform = [&](size_t off, size_t len, bool has_gang, int* ust, size_t* consumed) { return lt_uniform(e, off, len, has_gang, ust, consumed); };
+    bool on_device = false;                     // some results are in d_lt_res (a uniform run or a windowed stretch)
+    std::vector<std::pair<size_t, size_t>> in_host;   // the round stretches' [off, off + consumed): results in h_rd_res
+    auto uniform = [&](size_t off, size_t len, bool has_gang, int* ust, size_t* consumed) {
+        on_device = true;
+        return lt_uniform(e, off, len, has_gang, ust, consumed);
+    };
     auto window = [&](size_t off, size_t len, int* st, size_t* consumed) -> int {
+        on_device = true;
         if (!staged) {
             CK(cudaMemcpyAsync(e->d_lt_asks.p, e->h_lt_asks.p, 4 * B, cudaMemcpyHostToDevice, s));
             CK(cudaMemcpyAsync(e->d_lt_meta.p, e->h_lt_meta.p, 4 * B, cudaMemcpyHostToDevice, s));
@@ -761,17 +793,20 @@ int lt_batch(yk_engine* e, size_t B, int* status, size_t* done, std::vector<uint
             e->st.h2d_bytes += 4 * B;
             asks_staged = true;
         }
-        return lt_rounds(e, off, len, st, consumed);
+        const int rc = lt_rounds(e, off, len, st, consumed, [&](size_t o, size_t to) { ahead(e->h_rd_res.p, o, to); });
+        if (!rc) in_host.emplace_back(off, *consumed);
+        return rc;
     };
     const int rc = yklt::route_batch(e->cfg.policy == YK_POLICY_BINPACKING, !e->lt_force, e->cm.t, e->ord.insensitive, e->rd_taints,
                                      e->h_lt_asks.p, e->un_segs, e->h_lt_meta.p, uniform, rounds, window, status, done);
     if (rc) return rc;
-    if (*done) {
+    if (*done && on_device) {
         CK(cudaMemcpyAsync(e->h_lt_res.p, e->d_lt_res.p, 4 * *done, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
         e->st.d2h_bytes += 4 * *done;
     }
     result.assign(e->h_lt_res.p, e->h_lt_res.p + B);
+    for (const auto& r : in_host) std::copy(e->h_rd_res.p + r.first, e->h_rd_res.p + r.first + r.second, result.begin() + r.first);
     return YK_OK;
 }
 
@@ -780,15 +815,13 @@ int lt_export(yk_engine* e) {
     const int nlive = (int)e->nlive;
     if (nlive == 0) return YK_OK;
     cudaStream_t s = e->stream;
-    CK(cudaMemcpyAsync(e->h_flag.p, e->d_lt_cur.p, sizeof(int), cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    const int cur = e->h_flag[0] & 1;
-    yk_lt_export_kernel<<<(nlive + 255) / 256, 256, 0, s>>>(e->D, e->d_rec.p, e->lt_RS, e->d_ord[cur].p, nlive, e->d_avail.p, e->maxN);
+    yk_lt_export_kernel<<<(nlive + 255) / 256, 256, 0, s>>>(e->D, e->d_rec.p, e->lt_RS, e->d_ord[0].p, e->d_ord[1].p, e->d_lt_cur.p,
+                                                            nlive, e->d_avail.p, e->maxN);
     CK(cudaGetLastError());
     for (int k = 0; k < e->D; ++k)
         CK(cudaMemcpyAsync(e->n_avail.p + (size_t)k * e->maxN, e->d_avail.p + (size_t)k * e->maxN, 8 * (size_t)e->n_hi, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
-    e->st.d2h_bytes += 8 * (size_t)e->n_hi * e->D + 4;
+    e->st.d2h_bytes += 8 * (size_t)e->n_hi * e->D;
     e->st.other_launches += 1;
     return YK_OK;
 }
@@ -1163,8 +1196,9 @@ void yk_destroy(yk_engine* e) {
     if (e->stream) cudaStreamSynchronize(e->stream);
     if (e->hp_on && e->hp_n)
         fprintf(stderr, "[ykgpu] host ms per cycle (%llu cycles): prologue %.3f  upload+device_order %.3f  wait orderer setup %.3f  first fill + commit choice %.3f  "
-                        "run %.3f  epoch end / export + sync %.3f  finish %.3f\n", (unsigned long long)e->hp_n, e->hp[0] / e->hp_n, e->hp[1] / e->hp_n,
-                e->hp[2] / e->hp_n, e->hp[3] / e->hp_n, e->hp[4] / e->hp_n, e->hp[5] / e->hp_n, e->hp[6] / e->hp_n);
+                        "run %.3f (of which settling behind the round kernel %.3f)  epoch end / export + sync %.3f  finish %.3f\n",
+                (unsigned long long)e->hp_n, e->hp[0] / e->hp_n, e->hp[1] / e->hp_n, e->hp[2] / e->hp_n, e->hp[3] / e->hp_n, e->hp[4] / e->hp_n,
+                e->hp[7] / e->hp_n, e->hp[5] / e->hp_n, e->hp[6] / e->hp_n);
     if (e->lt_prof && e->d_lt_prof.p) {
         long long pf[32] = {0};
         if (cudaMemcpy(pf, e->d_lt_prof.p, sizeof(pf), cudaMemcpyDeviceToHost) == cudaSuccess) {
@@ -1285,6 +1319,7 @@ int yk_create(const yk_config* cfg, yk_engine** out) {
     if (const char* rw = getenv("YK_ROUND_WINDOW")) e->rd_window = std::max(1, std::min(atoi(rw), ykrd::WCAP));
     if (const char* rg = getenv("YK_ROUND_GUARD")) e->rd_guard = std::max(0, atoi(rg));
     T(e->d_rd_spent.alloc(N)); T(e->d_rd_req.alloc(A * (size_t)D)); T(e->d_rd_hdr.alloc(ykrd::R_WORDS)); T(e->h_rd_hdr.alloc(ykrd::R_WORDS));
+    T(e->h_rd_res.alloc(A, true)); T(e->h_rd_prog.alloc(1, true));
     T(e->d_lt_prof.alloc(32));   // [0, 16) the lattice kernel's phases, [16, 32) the round kernel's
     if (ok) T(cudaMemset(e->d_lt_prof.p, 0, 32 * sizeof(long long)));
     if (ok) T(lattice_setup(D, &e->lt_smem));
@@ -1642,9 +1677,14 @@ int run_lattice(yk_engine* e, Cycle& c, yklt::Choice& ch, bool& handoff) {
         CK(cudaStreamSynchronize(e->stream));
         if (e->h_flag[0]) return e->fail(YK_ERR_RANGE, "NaN node score (zero total on a weighted resource)");
     }
-    return yklt::device_commit(lp, [&](size_t B, int* status, size_t* consumed) { return lt_batch(e, B, status, consumed, c.result); },
-                               [&](uint32_t a, uint32_t node) { bind_one(e, c, a, node); },
-                               [&](int code, const char* m) { return e->fail(code, m); }, handoff);
+    auto bind = [&](uint32_t a, uint32_t node) { bind_one(e, c, a, node); };
+    auto ahead = [&](const uint32_t* res, size_t off, size_t to) { yklt::settle_ahead(lp, res, off, to, bind); };
+    auto batch = [&](size_t B, int* status, size_t* consumed) {
+        const int rcb = lt_batch(e, B, status, consumed, c.result, ahead);
+        if (rcb || *status == yklt::ST_NAN) yklt::settle_back(lp, [&](uint32_t a) { e->a_bound[a] = YK_NONE; --c.n; });
+        return rcb;
+    };
+    return yklt::device_commit(lp, batch, bind, [&](int code, const char* m) { return e->fail(code, m); }, handoff);
 }
 
 // The cycle on the sweep + host commit path.  slot[0] holds the first batch (filled, not yet launched); the host commit's

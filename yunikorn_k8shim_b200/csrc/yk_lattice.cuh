@@ -28,12 +28,13 @@ __global__ void yk_lt_init_kernel(int D, const int64_t* __restrict__ total, cons
     yklt::init_node(D, p, total, avail, ldn, taint, label, flags, rank, sorted_key, sorted_node, rec, RS, ord);
 }
 
-// available of every live node back into the column-major table (position order = any order: each node once)
-__global__ void yk_lt_export_kernel(int D, const int64_t* __restrict__ rec, int RS, const yklt::Ent* __restrict__ ord, int nlive,
-                                    int64_t* __restrict__ avail, size_t ldn) {
+// available of every live node back into the column-major table (position order = any order: each node once); the current
+// order buffer is ord[*cur & 1], read here so that the host need not wait for the commit to learn it
+__global__ void yk_lt_export_kernel(int D, const int64_t* __restrict__ rec, int RS, const yklt::Ent* ord0, const yklt::Ent* ord1,
+                                    const int* cur, int nlive, int64_t* __restrict__ avail, size_t ldn) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= nlive) return;
-    const uint32_t n = (uint32_t)ord[p].rn;
+    const uint32_t n = (uint32_t)((*cur & 1) ? ord1 : ord0)[p].rn;
     const int64_t* r = rec + (size_t)n * RS;
     for (int k = 0; k < D; ++k) avail[(size_t)k * ldn + n] = r[k];
 }

@@ -44,22 +44,11 @@ inline bool same_gang(const Tables& t, uint32_t x, uint32_t y) {
     return t.a_gang[x] != CNONE && t.a_gang[x] == t.a_gang[y] && t.a_app[x] == t.a_app[y];
 }
 
-// Decided entries [0, consumed) of a batch: orderer bookkeeping, and bind(ask, node) for every placement.  Returns whether
-// the batch ended on an ask / gang that found no node in a placement-sensitive order: the orderer is then rewound to just
-// before it (`later`, a batch filled after this one, is undone as well).
+// Decided entries [from, to) of a batch: orderer bookkeeping, and bind(ask, node) for every placement, in entry order.
 template <class Bind>
-inline bool settle(Orderer& ord, const std::vector<uint32_t>& asks, Orderer::Snap& snap, Orderer::Snap* later, const uint32_t* result,
-                   size_t consumed, bool ins, yk_stats_t& st, Bind&& bind) {
-    bool failed = false;
-    if (!ins && consumed > 0 && result[consumed - 1] == CNONE) {
-        const auto t0 = std::chrono::steady_clock::now();
-        size_t j = consumed - 1;   // first entry of the failed ask / gang
-        while (j > 0 && same_gang(ord.t, asks[j], asks[j - 1]) && result[j - 1] == CNONE) --j;
-        ord.rewind(snap, later, asks, j);
-        st.host_ms[2] += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-        failed = true;
-    }
-    for (size_t i = 0; i < consumed; ++i) {
+inline void settle_entries(Orderer& ord, const uint32_t* asks, const uint32_t* result, size_t from, size_t to, bool ins, yk_stats_t& st,
+                           Bind&& bind) {
+    for (size_t i = from; i < to; ++i) {
         const uint32_t a = asks[i];
         if (result[i] == CNONE) {
             if (ins) ord.fail_in_place(a);
@@ -70,6 +59,37 @@ inline bool settle(Orderer& ord, const std::vector<uint32_t>& asks, Orderer::Sna
         bind(a, result[i]);
         st.allocations++;
     }
+}
+
+// Takes back settle_entries over [0, to) of a batch in a placement-insensitive order, last entry first: every entry is in
+// flight again, and unbind(ask) takes back each binding.
+template <class Unbind>
+inline void unsettle_entries(Orderer& ord, const uint32_t* asks, size_t to, yk_stats_t& st, Unbind&& unbind) {
+    for (size_t i = to; i-- > 0;) {
+        const bool placed = ord.t.a_state[asks[i]] == ST_ALLOCATED;
+        ord.unconfirm(asks[i], placed);
+        if (placed) { unbind(asks[i]); st.allocations--; }
+        else st.nofit--;
+    }
+}
+
+// Decided entries [from, consumed) of a batch (settle_entries; [0, from) were settled while the batch was being decided,
+// which only a placement-insensitive order allows).  Returns whether the batch ended on an ask / gang that found no node in
+// a placement-sensitive order: the orderer is then rewound to just before it (`later`, a batch filled after this one, is
+// undone as well).
+template <class Bind>
+inline bool settle(Orderer& ord, const std::vector<uint32_t>& asks, Orderer::Snap& snap, Orderer::Snap* later, const uint32_t* result,
+                   size_t consumed, bool ins, yk_stats_t& st, Bind&& bind, size_t from = 0) {
+    bool failed = false;
+    if (!ins && consumed > 0 && result[consumed - 1] == CNONE) {
+        const auto t0 = std::chrono::steady_clock::now();
+        size_t j = consumed - 1;   // first entry of the failed ask / gang
+        while (j > 0 && same_gang(ord.t, asks[j], asks[j - 1]) && result[j - 1] == CNONE) --j;
+        ord.rewind(snap, later, asks, j);
+        st.host_ms[2] += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+        failed = true;
+    }
+    settle_entries(ord, asks.data(), result, from, consumed, ins, st, bind);
     return failed;
 }
 
@@ -551,12 +571,33 @@ struct Loop {
     size_t bmax;                                            // largest batch
     uint32_t max_bindings; const uint32_t& n;               // bindings allowed in the cycle, made so far
     yk_stats_t& st;
+    size_t settled = 0;                                     // entries of the batch settled while it was being decided
 };
 
+// Settles entries [lp.settled, to) of the batch being decided while the device still decides the rest: a round stretch
+// [off, ...) of a placement-insensitive order publishes its decided prefix (result, indexed like the batch), and no later
+// entry can undo it.  Only once every entry before the stretch is settled; the batch's own settle takes the rest.
+template <class Bind>
+inline void settle_ahead(Loop& lp, const uint32_t* result, size_t off, size_t to, Bind&& bind) {
+    if (!lp.ord.insensitive || lp.settled < off || to <= lp.settled) return;
+    yk::settle_entries(lp.ord, lp.asks.data(), result, lp.settled, to, true, lp.st, bind);
+    lp.settled = to;
+}
+
+// Takes back what settle_ahead settled of a batch that then fails (an error, or ST_NAN): no binding of a failed batch is
+// made; unbind(ask) takes back the last binding.
+template <class Unbind>
+inline void settle_back(Loop& lp, Unbind&& unbind) {
+    yk::unsettle_entries(lp.ord, lp.asks.data(), lp.settled, lp.st, unbind);
+    lp.settled = 0;
+}
+
 // The cycle on the device commit, batch by batch.  batch(B, &status, &consumed) decides one batch into lp.result[0,
-// consumed); bind(ask, node) takes a binding (and counts it in lp.n); fail(yk_status, message) reports an error.  Returns
-// with handoff = true, lp.asks holding the decided prefix only, when a gang has to be rolled back after a partial
-// placement: the rest of the cycle belongs to the host commit.
+// consumed); it may settle a prefix of it on the way (settle_ahead, into lp.settled), and a batch that fails (a non-zero
+// return or ST_NAN) must leave nothing settled (settle_back).  bind(ask, node) takes a binding (and counts it in lp.n);
+// fail(yk_status, message) reports an error.  Returns with handoff = true, lp.asks holding the decided prefix only, when a
+// gang has to be rolled back after a partial placement or the round guard ends a stretch: the rest of the cycle belongs to
+// the host commit.
 template <class Batch, class Bind, class Fail>
 inline int device_commit(Loop& lp, Batch&& batch, Bind&& bind, Fail&& fail, bool& handoff) {
     handoff = false;
@@ -571,6 +612,7 @@ inline int device_commit(Loop& lp, Batch&& batch, Bind&& bind, Fail&& fail, bool
         lp.plan_ready = false;
         size_t consumed = 0;
         int status = ST_DONE;
+        lp.settled = 0;
         if (lp.no_nodes) {   // nothing fits
             lp.result.assign(B, NONE);
             consumed = yk::no_node_consumed(lp.ord.t, lp.asks, ins);
@@ -588,12 +630,12 @@ inline int device_commit(Loop& lp, Batch&& batch, Bind&& bind, Fail&& fail, bool
             lp.result.resize(consumed);
             // no failure cut: every decided entry stands (a placement-sensitive batch never carries a NONE before a hand-over,
             // the kernel stops there instead; an insensitive one fails NONE entries in place)
-            yk::settle(lp.ord, lp.asks, lp.snap, nullptr, lp.result.data(), consumed, true, lp.st, bind);
+            yk::settle(lp.ord, lp.asks, lp.snap, nullptr, lp.result.data(), consumed, true, lp.st, bind, lp.settled);
             lp.st.lattice_handoffs++;
             handoff = true;
             return 0;
         }
-        const bool failed = yk::settle(lp.ord, lp.asks, lp.snap, nullptr, lp.result.data(), consumed, ins, lp.st, bind);
+        const bool failed = yk::settle(lp.ord, lp.asks, lp.snap, nullptr, lp.result.data(), consumed, ins, lp.st, bind, lp.settled);
         if (!failed && consumed < B) return fail(YK_ERR_CUDA, "lattice kernel ended a batch early without a failure");
         bsz = yk::next_batch_size(bsz, lp.bmax, failed);
         if (!yk::fill_batch(lp.ord, bsz, lp.bmax, (size_t)lp.max_bindings - lp.n, lp.asks, lp.snap, lp.st)) return fail(YK_ERR_ARG, yk::GANG_TOO_BIG);

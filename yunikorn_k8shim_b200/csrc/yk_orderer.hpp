@@ -408,6 +408,13 @@ public:
             for (int k = 0; k < t.D; ++k) ap[t.a_app[a]].alloc[k] += req(a, k);   // application's total once, in finish()
     }
 
+    // insensitive batches: undoes confirm(a) (placed) or fail_in_place(a); the ask is in flight again, in the state
+    // begin_cycle left it in (a gang member tentative, any other ask pending)
+    void unconfirm(uint32_t a, bool placed) {
+        t.a_state[a] = t.a_gang[a] != NONE ? ST_TENTATIVE : ST_PENDING;
+        if (placed) for (int k = 0; k < t.D; ++k) ap[t.a_app[a]].alloc[k] -= req(a, k);
+    }
+
     void finish() {   // persist queue and application allocations
         if (insensitive)   // gang members queued but never batched (max_bindings cut the cycle) are simply still pending
             for (size_t i = static_next; i < static_order.size(); ++i)

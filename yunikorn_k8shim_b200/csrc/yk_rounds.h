@@ -46,6 +46,7 @@ constexpr int GUARD_PASSES = 16;        // passes before the guard looks at the 
 // the guard's asks per pass: a pass costs 24-40 us at 2 000-10 000 nodes (H100, DESIGN.md §6.3), the host path 0.2-0.3 us
 // per ask, so a stretch that averages fewer asks per pass costs several times what the host path would
 constexpr int GUARD = 32;
+constexpr int PUBLISH_PASSES = 8;       // passes per publication of the decided count (Args::prog), a power of two
 
 // hdr[] words: asks decided, yklt::ST_*, passes, single steps, nodes that left the order
 enum { R_CONSUMED = 0, R_STATUS = 1, R_PASSES = 2, R_SINGLES = 3, R_SPENT = 4, R_WORDS = 5 };
@@ -64,6 +65,8 @@ struct Args {
                                            // (host: one is allocated when it is null)
     uint32_t* res;                         // [B] node index or NONE
     int* hdr;                              // [R_WORDS]
+    volatile int* prog;                    // device: asks decided so far, published every PUBLISH_PASSES passes for the host,
+                                           // which settles them while the stretch goes on (nullptr: off); never read here
     int window;                            // candidates per round, 1..WCAP
     int guard;                             // asks per pass below which the stretch ends (0: never)
     long long* prof;                       // optional [RP_N]: SM clocks per phase, accumulated by thread 0 (nullptr: off)
@@ -281,6 +284,19 @@ LT_FN void flush_side(const Args& a, Shared& s, int& buf, int& hd, int& n, int& 
     buf ^= 1; hd = 0; n += nl; nl = 0;
 }
 
+// Thread 0, after a barrier that follows the res writes of the asks [0, t): t for the host.  Called at the top of every
+// PUBLISH_PASSES-th pass; the passes after the last one come with the header.  The system-scope fence orders every thread's
+// res writes (made visible to thread 0 by the barrier) before the count, so a host that reads t with acquire semantics
+// reads their results too.  The fence waits for the pass's res writes to reach host memory, ~3 us on H100 (config 2: the
+// candidate phase grew by 6.5 k SM clocks per pass when every pass published), so it is paid once per 8 passes.
+LT_FN void publish(const Args& a, int t) {
+#if LT_DEV
+    if (a.prog && threadIdx.x == 0) { __threadfence_system(); *a.prog = t; }
+#else
+    (void)a; (void)t;
+#endif
+}
+
 // ---- the stretch -------------------------------------------------------------------------------------------------
 template <int D>
 LT_FN void stretch(const Args& a, Shared& s) {
@@ -342,6 +358,7 @@ LT_FN void stretch(const Args& a, Shared& s) {
     LT_PROF(RP_EDGES);
 
     while (t < B) {
+        if ((passes & (PUBLISH_PASSES - 1)) == 0) publish(a, t);   // (the res writes so far are behind the barriers that ended their passes)
         const int left = B - t;
         int W = a.window < left ? a.window : left;
         W = W < n_act + nl ? W : n_act + nl;

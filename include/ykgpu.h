@@ -177,6 +177,9 @@ typedef struct {
     /* round commit of the device commit (mask-free stretches decided in rounds at the front of the node order): passes
        (rounds and single steps), asks it decided, single steps (the front node rejected the ask) */
     uint64_t round_passes, round_asks, round_single_steps;
+    /* speculative round-commit launches (started on the device's own order of the cycle's asks before the host has set the
+       cycle up): adopted (the host's first batch and plan were exactly that launch), discarded (stopped; nothing it wrote read) */
+    uint64_t spec_adopted, spec_discarded;
 } yk_stats_t;
 
 int yk_create(const yk_config* cfg, yk_engine** out);

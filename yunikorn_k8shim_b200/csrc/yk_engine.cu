@@ -34,6 +34,7 @@
 #include "yk_lattice.cuh"
 #include "yk_uniform.cuh"
 #include "yk_rounds.cuh"
+#include "yk_spec.cuh"
 #include "yk_commit.hpp"
 #include "yk_lattice_host.hpp"
 #include "yk_orderer.hpp"
@@ -276,7 +277,7 @@ struct yk_engine {
     std::vector<uint8_t> a_cause;               // per ask: 0, ST_SLOWPATH or ST_INVALID (yk::Tables::a_cause), kept by yk_asks_upsert
     cudaEvent_t ev_l0 = nullptr, ev_l1 = nullptr;
     // uniform runs (yk_uniform.h): allocated on first use; element buffers hold UN_EMAX generated elements
-    bool hp_on = false; double hp[8] = {0, 0, 0, 0, 0, 0, 0, 0}; uint64_t hp_n = 0;
+    bool hp_on = false; double hp[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; uint64_t hp_n = 0;
     bool un_alloc = false, un_ord_stale = false;   // un_ord_stale: uniform runs moved nodes since d_ord was last written
     int un_min = 2048;                          // shortest run that takes the uniform path (YK_UNIFORM_MIN)
     int un_depth = 0;                           // first depth of a uniform run's attempt (YK_UNIFORM_DEPTH); 0: ykun::first_depth
@@ -296,6 +297,19 @@ struct yk_engine {
     // host reads while the kernel runs
     Pin<uint32_t> h_rd_res; Pin<int> h_rd_prog;
     Dev<int64_t> d_rd_req;                      // [maxA][D]: a stretch's requests in stretch order (ykrd::Args::sreq)
+    // speculative round-commit launch (yk_spec.h): device copies of what the static order needs (uploaded with the ask and
+    // application tables when they are stale; the ask states every cycle), the order's own sort buffers and the screen's
+    // words.  Mapped: the order and the words for the host's compare, and the abort word the kernel reads.
+    bool sp_asks_stale = true, sp_apps_stale = true;
+    bool sp_live = false;                       // a speculative launch of this cycle is on the stream
+    bool sp_adopt = false;                      // ... and the host adopted it: lt_rounds takes it instead of launching
+    std::vector<uint32_t> sp_pending;           // a speculative cycle's pending asks, listed on the calling thread
+    Dev<uint32_t> d_sp_app, d_sp_gang, d_sp_sig; Dev<int64_t> d_sp_create, d_sp_submit; Dev<int32_t> d_sp_prio;
+    Dev<uint8_t> d_sp_cause, d_sp_state, d_sp_present;
+    Dev<uint64_t> d_sp_ckey[2], d_sp_pkey[2]; Dev<uint32_t> d_sp_cval[2], d_sp_ukey[2], d_sp_pval[2], d_sp_pos, d_sp_brk[2], d_sp_w;
+    Dev<uint8_t> d_sp_cub; size_t sp_cub_bytes = 0;
+    Pin<uint8_t> h_sp_state; Pin<uint32_t> h_sp_order, h_sp_w, h_sp_init; Pin<int> h_sp_abort;
+    cudaEvent_t ev_sp = nullptr;                // after the screen: the order, the words and the NaN flag have landed
     Dev<uint32_t> pre_q; Dev<int64_t> pre_v; Dev<int32_t> pre_o;   // yk_preemption_search staging, grown on demand
     // yk_filter_nodes: its own node order (so a cycle's sort buffers are never touched) and per-chunk buffers, grown on demand
     Dev<uint64_t> f_key_in, f_key_out; Dev<uint32_t> f_val_in, f_val_out; Dev<uint8_t> f_cub; size_t f_cub_bytes = 0;
@@ -425,8 +439,29 @@ int upload_tables(yk_engine* e) {
         CK(cudaMemcpyAsync(e->d_adeny.p, e->a_deny.p, 8 * n, cudaMemcpyHostToDevice, e->stream));
         CK(cudaMemcpyAsync(e->d_anode.p, e->a_node.p, 4 * n, cudaMemcpyHostToDevice, e->stream));
         e->st.h2d_bytes += n * (8 * D + 28);
+        e->sp_asks_stale = true;
     }
     e->asks_stale = false;
+    // the speculative order's tables, where a cycle may start on the round commit (spec_gate)
+    if (e->lt_allowed && e->lt_auto && !e->lt_force && e->rd_min > 0 && e->un_min > 0) {
+        if (e->sp_asks_stale && e->a_hi) {
+            const size_t n = e->a_hi;
+            CK(cudaMemcpyAsync(e->d_sp_app.p, e->a_app.data(), 4 * n, cudaMemcpyHostToDevice, e->stream));
+            CK(cudaMemcpyAsync(e->d_sp_create.p, e->a_create.data(), 8 * n, cudaMemcpyHostToDevice, e->stream));
+            CK(cudaMemcpyAsync(e->d_sp_prio.p, e->a_prio.data(), 4 * n, cudaMemcpyHostToDevice, e->stream));
+            CK(cudaMemcpyAsync(e->d_sp_gang.p, e->a_gang.data(), 4 * n, cudaMemcpyHostToDevice, e->stream));
+            CK(cudaMemcpyAsync(e->d_sp_cause.p, e->a_cause.data(), n, cudaMemcpyHostToDevice, e->stream));
+            CK(cudaMemcpyAsync(e->d_sp_sig.p, e->a_sigid.data(), 4 * n, cudaMemcpyHostToDevice, e->stream));
+            e->st.h2d_bytes += n * 25;
+        }
+        if (e->sp_apps_stale) {
+            CK(cudaMemcpyAsync(e->d_sp_submit.p, e->p_submit.data(), 8 * (size_t)e->maxP, cudaMemcpyHostToDevice, e->stream));
+            CK(cudaMemcpyAsync(e->d_sp_present.p, e->p_present.data(), e->maxP, cudaMemcpyHostToDevice, e->stream));
+            e->st.h2d_bytes += 9 * (size_t)e->maxP;
+        }
+        if (e->sp_asks_stale || e->sp_apps_stale) CK(cudaStreamSynchronize(e->stream));   // the sources are pageable
+        e->sp_asks_stale = e->sp_apps_stale = false;
+    }
     return YK_OK;
 }
 
@@ -706,11 +741,11 @@ int lt_window(yk_engine* e, size_t off, size_t B) {
 // One round-eligible stretch [off, off + B) of the staged batch through yk_rounds_kernel.  Its results land in the mapped
 // h_rd_res at the same offset; while the kernel runs, ahead(off, to) is called for every newly published decided prefix
 // [off, to), which the caller settles behind the kernel (yklt::settle_ahead).
-template <class Ahead>
-int lt_rounds(yk_engine* e, size_t off, size_t B, int* status, size_t* consumed, Ahead&& ahead) {
+// The round kernel over the staged stretch [off, off + B) (a.go etc. null), with its events and the header's read-back
+int launch_stretch(yk_engine* e, size_t off, size_t B, const ykrd::Args* spec = nullptr) {
     cudaStream_t s = e->stream;
-    { const int rco = un_reorder(e); if (rco) return rco; }
     ykrd::Args a{};
+    if (spec) a = *spec;
     a.policy = e->cfg.policy;
     for (int k = 0; k < 8; ++k) a.w[k] = e->w.w[k];
     a.rec = e->d_rec.p; a.RS = e->lt_RS; a.ord[0] = e->d_ord[0].p; a.ord[1] = e->d_ord[1].p; a.cur = e->d_lt_cur.p;
@@ -726,6 +761,17 @@ int lt_rounds(yk_engine* e, size_t off, size_t B, int* status, size_t* consumed,
     CK(cudaGetLastError());
     CK(cudaEventRecord(e->ev_l1, s));
     CK(cudaMemcpyAsync(e->h_rd_hdr.p, e->d_rd_hdr.p, ykrd::R_WORDS * sizeof(int), cudaMemcpyDeviceToHost, s));
+    return YK_OK;
+}
+
+template <class Ahead>
+int lt_rounds(yk_engine* e, size_t off, size_t B, int* status, size_t* consumed, Ahead&& ahead) {
+    cudaStream_t s = e->stream;
+    { const int rco = un_reorder(e); if (rco) return rco; }
+    // an adopted speculative launch (spec_verify) is this stretch, the batch's only one, already running
+    const bool adopted = e->sp_adopt && off == 0;
+    e->sp_adopt = false;
+    if (!adopted) { const int rcl = launch_stretch(e, off, B); if (rcl) return rcl; }
     // settle behind the kernel until it ends; the count is read after the query, so the last pass sees its final value.  The
     // kernel never waits for the host: this loop only reads.
     for (size_t seen = 0;;) {
@@ -762,7 +808,8 @@ template <class Ahead>
 int lt_batch(yk_engine* e, size_t B, int* status, size_t* done, std::vector<uint32_t>& result, Ahead&& ahead) {
     cudaStream_t s = e->stream;
     memcpy(e->h_lt_asks.p, e->slot[0].asks.data(), 4 * B);
-    bool staged = false, asks_staged = false;   // only the windowed kernel reads the per-entry words, the round kernel the asks
+    bool staged = false, asks_staged = e->sp_adopt;   // only the windowed kernel reads the per-entry words, the round kernel the
+                                                       // asks (an adopted speculative launch wrote them itself)
     bool on_device = false;                     // some results are in d_lt_res (a uniform run or a windowed stretch)
     std::vector<std::pair<size_t, size_t>> in_host;   // the round stretches' [off, off + consumed): results in h_rd_res
     auto uniform = [&](size_t off, size_t len, bool has_gang, int* ust, size_t* consumed) {
@@ -823,6 +870,105 @@ int lt_export(yk_engine* e) {
     CK(cudaStreamSynchronize(s));
     e->st.d2h_bytes += 8 * (size_t)e->n_hi * e->D;
     e->st.other_launches += 1;
+    return YK_OK;
+}
+
+// ---- speculative round-commit launch (yk_spec.h, DESIGN.md §6.3) ----------------------------------------------------
+// Cheap host gates, O(applications + queues), before the pending scan: a cycle under `auto` on the fair sort whose order can
+// be placement-insensitive -- every present application in one fifo leaf with no max on its chain, no user limit, no queue
+// priority offset or fence -- and with enough asks for the round commit.
+bool spec_gate(const yk_engine* e, uint32_t max_bindings, bool auto_lattice) {
+    if (!auto_lattice || e->cfg.policy != YK_POLICY_FAIR || e->rd_min <= 0 || max_bindings == 0 || e->a_hi < (uint32_t)e->rd_min || e->n_ul)
+        return false;
+    uint32_t leaf = YK_NONE;
+    for (uint32_t p = 0; p < e->maxP; ++p) {
+        if (!e->p_present[p]) continue;
+        if (leaf == YK_NONE) leaf = e->p_queue[p];
+        else if (e->p_queue[p] != leaf) return false;
+    }
+    if (leaf == YK_NONE || e->q_sort[leaf] != 0) return false;
+    for (uint32_t q = 0; q < e->nq; ++q)
+        if ((q > 0 && e->q_parent[q] == leaf) || e->q_prio_offset[q] != 0 || e->q_prio_fence[q]) return false;
+    for (uint32_t q = leaf; q != YK_NONE; q = e->q_parent[q])
+        for (int k = 0; k < e->D; ++k) if (e->q_max[(size_t)k * e->nq + q] != yk::UNSET) return false;
+    return true;
+}
+
+// Enqueues, behind device_order: the static order of the kept asks into d_lt_asks (and h_sp_order), the screen, lt_prepare's
+// set-up and the round kernel over the order, which returns at once unless the screen said GO and no node scores NaN.
+// h_sp_state holds the ask states as the cycle began.  Needs the tables uploaded and the node order enqueued.
+int spec_launch(yk_engine* e, uint32_t max_bindings) {
+    if (!e->nlive || !e->ranks_unique) return YK_OK;
+    for (int k = 0; k < e->D; ++k) if (!(e->w.w[k] >= 0.0)) return YK_OK;
+    cudaStream_t s = e->stream;
+    const uint32_t A = e->a_hi, P = e->maxP, n = std::max(std::max(A, e->nlive), P);
+    CK(cudaMemcpyAsync(e->d_sp_state.p, e->h_sp_state.p, A, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(e->d_sp_w.p, e->h_sp_init.p, 4 * ykspec::W_N, cudaMemcpyHostToDevice, s));
+    e->st.h2d_bytes += A + 4 * ykspec::W_N;
+    yk_spec_scan_kernel<<<(n + 255) / 256, 256, 0, s>>>(A, e->d_sp_state.p, e->d_sp_app.p, e->d_sp_create.p, e->d_sp_prio.p,
+        e->d_sp_gang.p, e->d_sp_cause.p, e->d_atol.p, e->d_aneed.p, e->d_adeny.p, e->d_anode.p, e->d_sp_present.p, P,
+        e->d_sp_submit.p, e->nlive, e->d_by_rank.p, e->d_taint.p, e->d_sp_ckey[0].p, e->d_sp_cval[0].p, e->d_sp_pkey[0].p,
+        e->d_sp_pval[0].p, e->d_sp_w.p);
+    CK(cudaGetLastError());
+    size_t tb = e->sp_cub_bytes;
+    CK(cub::DeviceRadixSort::SortPairs(e->d_sp_cub.p, tb, e->d_sp_pkey[0].p, e->d_sp_pkey[1].p, e->d_sp_pval[0].p, e->d_sp_pval[1].p, (int)P, 0, 64, s));
+    yk_spec_pos_kernel<<<(P + 255) / 256, 256, 0, s>>>(P, e->d_sp_pval[1].p, e->d_sp_pos.p);
+    tb = e->sp_cub_bytes;
+    CK(cub::DeviceRadixSort::SortPairs(e->d_sp_cub.p, tb, e->d_sp_ckey[0].p, e->d_sp_ckey[1].p, e->d_sp_cval[0].p, e->d_sp_cval[1].p, (int)A, 0, 64, s));
+    yk_spec_appkey_kernel<<<(A + 255) / 256, 256, 0, s>>>(A, e->d_sp_cval[1].p, e->d_sp_state.p, e->d_sp_app.p, e->d_sp_cause.p,
+                                                         e->d_sp_present.p, e->d_sp_pos.p, P, e->d_sp_ukey[0].p);
+    int bits = 1;
+    while (bits < 32 && (1ull << bits) <= P) ++bits;
+    tb = e->sp_cub_bytes;
+    CK(cub::DeviceRadixSort::SortPairs(e->d_sp_cub.p, tb, e->d_sp_ukey[0].p, e->d_sp_ukey[1].p, e->d_sp_cval[1].p, e->d_lt_asks.p, (int)A, 0, bits, s));
+    yk_spec_break_kernel<<<(A + 255) / 256, 256, 0, s>>>(A, e->d_lt_asks.p, e->d_sp_sig.p, e->d_sp_w.p, max_bindings, e->d_sp_brk[0].p, e->h_sp_order.d);
+    tb = e->sp_cub_bytes;
+    CK(cub::DeviceScan::InclusiveSum(e->d_sp_cub.p, tb, e->d_sp_brk[0].p, e->d_sp_brk[1].p, (int)A, s));
+    yk_spec_run_kernel<<<(A + 255) / 256, 256, 0, s>>>(A, e->d_sp_brk[1].p, e->un_min, max_bindings, e->d_sp_w.p);
+    yk_spec_decide_kernel<<<1, 1, 0, s>>>(e->d_sp_w.p, (uint32_t)e->rd_min, max_bindings, e->h_sp_w.d);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(e->ev_sp, s));
+    e->st.other_launches += 6 + 3 * 10 + 3;   // six kernels, three cub sorts, one cub scan
+    int rc = lt_prepare(e);
+    if (rc) return rc;
+    ykrd::Args sp{};
+    sp.go = e->d_sp_w.p; sp.nan = e->d_flag.p; sp.abort = e->h_sp_abort.d;
+    rc = launch_stretch(e, 0, 0, &sp);
+    if (rc) return rc;
+    e->sp_live = true;
+    return YK_OK;
+}
+
+// A speculative launch that will not be used: the kernel stops at its next publication, and nothing it wrote is read (the
+// next launch or lt_prepare rebuilds records, order and results; its time and passes are never counted).
+int spec_discard(yk_engine* e) {
+    if (!e->sp_live) return YK_OK;
+    e->sp_live = false;
+    __atomic_store_n(e->h_sp_abort.p, 1, __ATOMIC_RELEASE);
+    const cudaError_t r = cudaStreamSynchronize(e->stream);
+    __atomic_store_n(e->h_sp_abort.p, 0, __ATOMIC_RELEASE);
+    e->st.spec_discarded++;
+    return r == cudaSuccess ? YK_OK : e->cuda_fail(r, "cudaStreamSynchronize (speculative launch)");
+}
+
+// After the commit choice: the speculative launch is adopted only when the host's own choice is exactly what it runs -- the
+// device commit, planned as one round-eligible stretch over the whole first batch, whose asks equal the device's order
+// element for element.  Otherwise it is discarded.
+int spec_verify(yk_engine* e, const yklt::Choice& ch) {
+    if (!e->sp_live) return YK_OK;
+    CK(cudaEventSynchronize(e->ev_sp));
+    const uint32_t* w = e->h_sp_w.p;
+    const std::vector<uint32_t>& asks = e->slot[0].asks;
+    const size_t B = asks.size();
+    const std::vector<ykun::Segment>& sg = e->un_segs;
+    const bool adopt = ch.device && ch.plan_ready && ch.rounds_only && w[ykspec::W_STATUS] == ykspec::GO && w[ykspec::W_COUNT] == B &&
+                       sg.size() == 1 && sg[0].off == 0 && (size_t)sg[0].len == B &&
+                       memcmp(asks.data(), e->h_sp_order.p, 4 * B) == 0;
+    if (!adopt) return spec_discard(e);
+    e->sp_live = false;
+    e->sp_adopt = true;
+    e->st.spec_adopted++;
+    e->st.d2h_bytes += 4 * B;
     return YK_OK;
 }
 
@@ -1195,10 +1341,11 @@ void yk_destroy(yk_engine* e) {
     e->worker.stop();
     if (e->stream) cudaStreamSynchronize(e->stream);
     if (e->hp_on && e->hp_n)
-        fprintf(stderr, "[ykgpu] host ms per cycle (%llu cycles): prologue %.3f  upload+device_order %.3f  wait orderer setup %.3f  first fill + commit choice %.3f  "
-                        "run %.3f (of which settling behind the round kernel %.3f)  epoch end / export + sync %.3f  finish %.3f\n",
-                (unsigned long long)e->hp_n, e->hp[0] / e->hp_n, e->hp[1] / e->hp_n, e->hp[2] / e->hp_n, e->hp[3] / e->hp_n, e->hp[4] / e->hp_n,
-                e->hp[7] / e->hp_n, e->hp[5] / e->hp_n, e->hp[6] / e->hp_n);
+        fprintf(stderr, "[ykgpu] host ms per cycle (%llu cycles): prologue %.3f  upload+device_order+speculative launch and hints %.3f  wait orderer setup %.3f  "
+                        "first fill + commit choice %.3f  verify speculative launch %.3f  run %.3f (of which settling behind the round kernel %.3f)  "
+                        "epoch end / export + sync %.3f  finish %.3f\n",
+                (unsigned long long)e->hp_n, e->hp[0] / e->hp_n, e->hp[1] / e->hp_n, e->hp[2] / e->hp_n, e->hp[3] / e->hp_n, e->hp[8] / e->hp_n,
+                e->hp[4] / e->hp_n, e->hp[7] / e->hp_n, e->hp[5] / e->hp_n, e->hp[6] / e->hp_n);
     if (e->lt_prof && e->d_lt_prof.p) {
         long long pf[32] = {0};
         if (cudaMemcpy(pf, e->d_lt_prof.p, sizeof(pf), cudaMemcpyDeviceToHost) == cudaSuccess) {
@@ -1223,6 +1370,7 @@ void yk_destroy(yk_engine* e) {
     if (e->ep_s1) cudaEventDestroy(e->ep_s1);
     if (e->ev_l0) cudaEventDestroy(e->ev_l0);
     if (e->ev_l1) cudaEventDestroy(e->ev_l1);
+    if (e->ev_sp) cudaEventDestroy(e->ev_sp);
     for (Slot& sl : e->slot) {
         for (auto ev : sl.ev) if (ev) cudaEventDestroy(ev);
         if (sl.ev_s0) cudaEventDestroy(sl.ev_s0);
@@ -1320,6 +1468,26 @@ int yk_create(const yk_config* cfg, yk_engine** out) {
     if (const char* rg = getenv("YK_ROUND_GUARD")) e->rd_guard = std::max(0, atoi(rg));
     T(e->d_rd_spent.alloc(N)); T(e->d_rd_req.alloc(A * (size_t)D)); T(e->d_rd_hdr.alloc(ykrd::R_WORDS)); T(e->h_rd_hdr.alloc(ykrd::R_WORDS));
     T(e->h_rd_res.alloc(A, true)); T(e->h_rd_prog.alloc(1, true));
+    T(e->d_sp_app.alloc(A)); T(e->d_sp_gang.alloc(A)); T(e->d_sp_sig.alloc(A)); T(e->d_sp_create.alloc(A)); T(e->d_sp_prio.alloc(A));
+    T(e->d_sp_cause.alloc(A)); T(e->d_sp_state.alloc(A)); T(e->d_sp_submit.alloc(e->maxP)); T(e->d_sp_present.alloc(e->maxP));
+    for (int b = 0; b < 2; ++b) {
+        T(e->d_sp_ckey[b].alloc(A)); T(e->d_sp_cval[b].alloc(A)); T(e->d_sp_ukey[b].alloc(A)); T(e->d_sp_brk[b].alloc(A));
+        T(e->d_sp_pkey[b].alloc(e->maxP)); T(e->d_sp_pval[b].alloc(e->maxP));
+    }
+    T(e->d_sp_pos.alloc(e->maxP)); T(e->d_sp_w.alloc(ykspec::W_N));
+    T(e->h_sp_state.alloc(A)); T(e->h_sp_order.alloc(A, true)); T(e->h_sp_w.alloc(ykspec::W_N, true)); T(e->h_sp_init.alloc(ykspec::W_N));
+    T(e->h_sp_abort.alloc(1, true));
+    T(cudaEventCreateWithFlags(&e->ev_sp, cudaEventDisableTiming));
+    if (ok) {
+        size_t b1 = 0, b2 = 0, b3 = 0, b4 = 0;
+        T(cub::DeviceRadixSort::SortPairs(nullptr, b1, e->d_sp_ckey[0].p, e->d_sp_ckey[1].p, e->d_sp_cval[0].p, e->d_sp_cval[1].p, (int)A, 0, 64, e->stream));
+        T(cub::DeviceRadixSort::SortPairs(nullptr, b2, e->d_sp_pkey[0].p, e->d_sp_pkey[1].p, e->d_sp_pval[0].p, e->d_sp_pval[1].p, (int)e->maxP, 0, 64, e->stream));
+        T(cub::DeviceRadixSort::SortPairs(nullptr, b3, e->d_sp_ukey[0].p, e->d_sp_ukey[1].p, e->d_sp_cval[1].p, e->d_lt_asks.p, (int)A, 0, 32, e->stream));
+        T(cub::DeviceScan::InclusiveSum(nullptr, b4, e->d_sp_brk[0].p, e->d_sp_brk[1].p, (int)A, e->stream));
+        e->sp_cub_bytes = std::max(std::max(b1, b2), std::max(b3, b4));
+        T(e->d_sp_cub.alloc(e->sp_cub_bytes));
+        e->h_sp_init[ykspec::W_PRIO_MIN] = 0xFFFFFFFFu;   // every other word starts at 0
+    }
     T(e->d_lt_prof.alloc(32));   // [0, 16) the lattice kernel's phases, [16, 32) the round kernel's
     if (ok) T(cudaMemset(e->d_lt_prof.p, 0, 32 * sizeof(long long)));
     if (ok) T(lattice_setup(D, &e->lt_smem));
@@ -1459,6 +1627,7 @@ int yk_apps_upsert(yk_engine* e, uint32_t n, const uint32_t* idx, const uint32_t
         if (!e->p_present[idx[i]]) for (int k = 0; k < e->D; ++k) e->p_alloc[(size_t)k * e->maxP + idx[i]] = 0;
         e->p_queue[idx[i]] = queue[i]; e->p_submit[idx[i]] = submit[i]; e->p_present[idx[i]] = 1;
     }
+    if (n) e->sp_apps_stale = true;
     return YK_OK;
 }
 
@@ -1492,6 +1661,7 @@ int yk_apps_remove(yk_engine* e, uint32_t n, const uint32_t* idx) {
         if (idx[i] >= e->maxP) return e->fail(YK_ERR_ARG, "yk_apps_remove: index beyond max_apps");
         e->p_present[idx[i]] = 0;
     }
+    if (n) e->sp_apps_stale = true;
     return YK_OK;
 }
 
@@ -1647,6 +1817,27 @@ int yk_asks_resize(yk_engine* e, uint32_t n, const uint32_t* idx, const int64_t*
 // ---- one cycle ---------------------------------------------------------------------------------------------------
 namespace {
 
+// How many distinct signatures do the cycle's pending asks (in index order) have?  Few: every one is swept once per epoch
+// (ep_local = its row), no per-batch device work at all
+void epoch_rows(yk_engine* e, const std::vector<uint32_t>& pend) {
+    e->ep_rows = false;
+    if (!e->share_rows || e->cfg.world > 1 || getenv("YK_NO_EPOCH_ROWS")) return;
+    if (e->ep_seen.size() < e->sigs.n) { e->ep_seen.assign(e->sigs.n + 1024, 0); e->ep_local.assign(e->sigs.n + 1024, 0); e->ep_stamp = 0; }
+    if (++e->ep_stamp == 0) { std::fill(e->ep_seen.begin(), e->ep_seen.end(), 0); e->ep_stamp = 1; }
+    e->ep_reps.clear();
+    uint32_t ns = 0;
+    for (uint32_t a : pend) {
+        const uint32_t id = e->a_sigid[a];
+        if (e->ep_seen[id] != e->ep_stamp) {
+            e->ep_seen[id] = e->ep_stamp;
+            if (ns < yk_engine::EP_MAX) { e->ep_local[id] = ns; e->ep_reps.push_back(a); }
+            if (++ns > yk_engine::EP_MAX) break;
+        }
+    }
+    e->ep_rows = ns > 0 && ns <= yk_engine::EP_MAX && (uint64_t)ns * 8 <= pend.size();
+    e->ep_n = ns;
+}
+
 struct Cycle {
     uint32_t max_bindings = 0;
     yk_binding* out = nullptr;
@@ -1665,7 +1856,7 @@ void bind_one(yk_engine* e, Cycle& c, uint32_t a, uint32_t node) {
 // true when the rest of the cycle belongs to the host commit.
 int run_lattice(yk_engine* e, Cycle& c, yklt::Choice& ch, bool& handoff) {
     handoff = false;
-    int rc = lt_prepare(e);
+    int rc = e->sp_adopt ? YK_OK : lt_prepare(e);   // an adopted speculative launch runs on what spec_launch prepared
     if (rc) return rc;
     Slot& A = e->slot[0];
     yklt::Loop lp{e->ord, e->cm.t, ch.shape_ids, e->a_sigid.data(), A.asks, A.snap, c.result,
@@ -1674,7 +1865,9 @@ int run_lattice(yk_engine* e, Cycle& c, yklt::Choice& ch, bool& handoff) {
                   e->ord.insensitive ? (size_t)e->maxA : (size_t)e->batch, c.max_bindings, c.n, e->st};
     if (e->nlive && !A.asks.empty()) {   // the initial order's NaN flag (device_order) is checked before the first batch
                                           // commits anything: a failed cycle must leave the node tables as they were
-        CK(cudaStreamSynchronize(e->stream));
+        // (an adopted launch is still running: the flag landed before the screen's event, and the kernel did nothing on NaN)
+        if (e->sp_adopt) CK(cudaEventSynchronize(e->ev_sp));
+        else CK(cudaStreamSynchronize(e->stream));
         if (e->h_flag[0]) return e->fail(YK_ERR_RANGE, "NaN node score (zero total on a weighted resource)");
     }
     auto bind = [&](uint32_t a, uint32_t node) { bind_one(e, c, a, node); };
@@ -1753,12 +1946,17 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
     const bool force_lattice = e->lt_allowed && e->lt_force && dev_policy;
     const bool auto_lattice = e->lt_allowed && !e->lt_force && e->lt_auto && e->un_min > 0 && dev_policy;
     yklt::Scan scan;   // the pending scan's hints for the commit choice
+    // a speculative round-commit launch reads the ask states as the cycle began: copied before the pending scan rewrites them
+    const bool spec = spec_gate(e, max_bindings, auto_lattice);
+    if (spec) memcpy(e->h_sp_state.p, e->a_state.data(), e->a_hi);
+    e->sp_live = e->sp_adopt = false;
     e->worker.submit([&] {
         const double t_b = now_ms();
         pending.clear();
         pending.reserve(e->a_hi);
         bool any_gang = false;
-        if (auto_lattice) for (uint32_t n = 0; n < e->n_hi; ++n) if (e->n_present[n]) scan.taints |= e->n_taint[n];
+        const bool hints = auto_lattice && !spec;   // (a speculative cycle's calling thread takes them: below)
+        if (hints) for (uint32_t n = 0; n < e->n_hi; ++n) if (e->n_present[n]) scan.taints |= e->n_taint[n];
         for (uint32_t a = 0; a < e->a_hi; ++a) {
             uint8_t& st = e->a_state[a];
             if (st == yk::ST_ABSENT || st == yk::ST_ALLOCATED) continue;
@@ -1766,10 +1964,10 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
             if (!e->p_present[e->a_app[a]]) continue;
             pending.push_back(a);
             any_gang = any_gang || e->a_gang[a] != YK_NONE;
-            if (auto_lattice) scan.add(e->cm.t, e->a_sigid.data(), a);
+            if (hints) scan.add(e->cm.t, e->a_sigid.data(), a);
         }
         e->cycle_has_gang = any_gang;
-        e->rd_taints = scan.taints;
+        if (!spec) e->rd_taints = scan.taints;
         if (any_gang) {   // a gang that no batch can hold is an argument error: found before anything is committed
             std::unordered_map<uint64_t, uint32_t> members;
             for (uint32_t a : pending)
@@ -1786,26 +1984,8 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
         t.p_user = e->p_user.data(); t.n_ul = e->n_ul; t.ul_queue = e->ul_queue.data(); t.ul_user = e->ul_user.data();
         t.ul_max = e->ul_max.data(); t.ul_alloc = e->ul_alloc.data();
         if (!gang_too_big) e->ord.begin_cycle(pending);
-        e->ep_rows = false;
-        if (!gang_too_big && e->share_rows && e->cfg.world <= 1 && !getenv("YK_NO_EPOCH_ROWS")) {
-            // how many distinct signatures do the pending asks have?  Few: every one is swept once per epoch (ep_local =
-            // its row), no per-batch device work at all
-            if (e->ep_seen.size() < e->sigs.n) { e->ep_seen.assign(e->sigs.n + 1024, 0); e->ep_local.assign(e->sigs.n + 1024, 0); e->ep_stamp = 0; }
-            if (++e->ep_stamp == 0) { std::fill(e->ep_seen.begin(), e->ep_seen.end(), 0); e->ep_stamp = 1; }
-            e->ep_reps.clear();
-            uint32_t ns = 0;
-            for (uint32_t a : pending) {
-                const uint32_t id = e->a_sigid[a];
-                if (e->ep_seen[id] != e->ep_stamp) {
-                    e->ep_seen[id] = e->ep_stamp;
-                    if (ns < yk_engine::EP_MAX) { e->ep_local[id] = ns; e->ep_reps.push_back(a); }
-                    if (++ns > yk_engine::EP_MAX) break;
-                }
-            }
-            e->ep_rows = ns > 0 && ns <= yk_engine::EP_MAX && (uint64_t)ns * 8 <= pending.size();
-            e->ep_n = ns;
-        }
-        if (!gang_too_big) scan.done(e->cm.t, pending, force_lattice, e->a_shape);
+        if (!gang_too_big && !spec) epoch_rows(e, pending);
+        if (!gang_too_big && !spec) scan.done(e->cm.t, pending, force_lattice, e->a_shape);
         e->ep_uploaded = false; e->ep_landed = true;
         begin_ms = now_ms() - t_b;
     });
@@ -1814,14 +1994,35 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
     // the device scores and sorts the nodes while the helper thread still sets the orderer up
     e->order_enqueued = false;
     if (!rc) { rc = device_order(e); e->order_enqueued = rc == YK_OK && e->nlive > 0; }
+    // ... and, where the cycle may be a round-commit one, orders the asks and starts the round kernel on them
+    if (!rc && spec) rc = spec_launch(e, max_bindings);
+    // ... and takes over the pending scan's commit-choice hints and the epoch rows, which read only which asks the scan keeps
+    // (the states as the cycle began, the present applications): they run next to the helper's orderer set-up, not after it
+    if (spec) {
+        std::vector<uint32_t>& kept = e->sp_pending;
+        kept.clear();
+        for (uint32_t n = 0; n < e->n_hi; ++n) if (e->n_present[n]) scan.taints |= e->n_taint[n];
+        for (uint32_t a = 0; a < e->a_hi; ++a) {
+            const uint8_t st = e->h_sp_state[a];
+            if (st == yk::ST_ABSENT || st == yk::ST_ALLOCATED || !e->p_present[e->a_app[a]]) continue;
+            kept.push_back(a);
+            scan.add(e->cm.t, e->a_sigid.data(), a);
+        }
+        e->rd_taints = scan.taints;
+        epoch_rows(e, kept);
+    }
     const double t_a = now_ms();
     hp(1);
     e->worker.wait();
     hp(2);
     e->st.host_ms[0] += t_a - t_start;
     e->st.host_ms[1] += begin_ms;
-    if (rc) return rc;
-    if (gang_too_big) return e->fail(YK_ERR_ARG, yk::GANG_TOO_BIG);
+    if (spec && !gang_too_big) scan.done(e->cm.t, pending, force_lattice, e->a_shape);
+    if (rc || gang_too_big) {
+        const int rcd = spec_discard(e);
+        if (rc) return rc;
+        return rcd ? rcd : e->fail(YK_ERR_ARG, yk::GANG_TOO_BIG);
+    }
 
     Cycle c;
     c.max_bindings = max_bindings; c.out = out;
@@ -1836,6 +2037,11 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
     if (!yklt::choose_commit(in, choice)) rc = e->fail(YK_ERR_ARG, yk::GANG_TOO_BIG);
     e->lt_active = false;
     hp(3);
+    {
+        const int rcv = rc ? spec_discard(e) : spec_verify(e, choice);
+        if (!rc) rc = rcv;
+    }
+    hp(8);
     if (!rc) {
         if (choice.device) {
             e->lt_active = true;
@@ -1865,6 +2071,7 @@ extern "C" int yk_cycle(yk_engine* e, uint32_t max_bindings, yk_binding* out, ui
         }
     }
     hp(4);
+    e->sp_adopt = false;
     // ---- always: leave host and device node tables current, persist what was bound, no ask left in flight ----
     int rc_end = YK_OK;
     if (e->lt_active) { rc_end = lt_export(e); e->lt_active = false; }

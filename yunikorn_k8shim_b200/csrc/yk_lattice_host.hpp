@@ -476,6 +476,7 @@ struct Choice {
     bool device = false;                  // the cycle starts on the device commit, else on the host commit
     const uint32_t* shape_ids = nullptr;  // build_meta's shape numbers: a_shape when forced, the signature ids under auto
     bool plan_ready = false;              // meta, shp, sig and segs already describe the first batch
+    bool rounds_only = false;             // ... and every segment of that plan is a round-eligible stretch (the cost rule's test)
 };
 
 // Which commit the cycle starts on, and its first batch (filled into in.asks, not launched).  Forced: the device commit
@@ -536,6 +537,7 @@ inline bool choose_commit(const ChoiceIn& in, Choice& out) {
             }
             else for (const ykun::Segment& sg : in.segs) {
                 const bool rounds = !sg.uniform && round_eligible(in.ct, ins, in.scan.taints, in.asks.data() + sg.off, (size_t)sg.len);
+                out.rounds_only = (&sg == in.segs.data() || out.rounds_only) && rounds;
                 dev_us += sg.uniform ? 250.0 : (rounds ? RD_US_PER_ASK : 0.35) * sg.len;
                 host_us += (rounds ? RD_HOST_US_PER_ASK : 0.7 * 0.08) * sg.len;
             }

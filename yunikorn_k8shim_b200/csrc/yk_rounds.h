@@ -28,6 +28,7 @@
 #include <assert.h>
 #include <stdint.h>
 #include "yk_lattice.h"
+#include "yk_spec.h"
 #if !LT_DEV
 #include <vector>
 #endif
@@ -48,8 +49,11 @@ constexpr int GUARD_PASSES = 16;        // passes before the guard looks at the 
 constexpr int GUARD = 32;
 constexpr int PUBLISH_PASSES = 8;       // passes per publication of the decided count (Args::prog), a power of two
 
-// hdr[] words: asks decided, yklt::ST_*, passes, single steps, nodes that left the order
+// hdr[] words: asks decided, yklt::ST_* or ST_ABORTED, passes, single steps, nodes that left the order
 enum { R_CONSUMED = 0, R_STATUS = 1, R_PASSES = 2, R_SINGLES = 3, R_SPENT = 4, R_WORDS = 5 };
+// a speculative launch (Args::go) that did not run, or stopped because the host set Args::abort: the host reads nothing
+// it wrote
+constexpr int ST_ABORTED = 4;
 
 struct Args {
     uint32_t policy;
@@ -70,11 +74,16 @@ struct Args {
     int window;                            // candidates per round, 1..WCAP
     int guard;                             // asks per pass below which the stretch ends (0: never)
     long long* prof;                       // optional [RP_N]: SM clocks per phase, accumulated by thread 0 (nullptr: off)
+    // a speculative launch (yk_spec.h), started before the host knows the stretch: go[ykspec::W_STATUS] is the screen's
+    // status and go[ykspec::W_COUNT] replaces B; the kernel returns at once unless the status is ykspec::GO and the node
+    // order's NaN flag (*nan) is clear.  abort: a host word in mapped memory, read with each publication; once set, the
+    // stretch ends with ST_ABORTED.  All three nullptr for a launch of a known stretch.
+    const uint32_t* go; const int* nan; const volatile int* abort;
 };
 enum { RP_EDGES = 0, RP_CAND, RP_SCAN, RP_APPLY, RP_SORT, RP_MERGE, RP_SINGLE, RP_N };   // stretch set-up + restore, then per round
 
 struct Shared {
-    int m, n_new, n_sp, hit, nan, keep;
+    int m, n_new, n_sp, hit, nan, keep, stop, B;   // B: the stretch's length (Args::B, or the speculative launch's count)
     long long prof_t;
     int64_t minreq[8];
     u64 ck[WCAP], cr[WCAP];                // candidate j: the new entry of S[j] after ask i+j (KEY_INF: S[j] rejects it)
@@ -289,18 +298,28 @@ LT_FN void flush_side(const Args& a, Shared& s, int& buf, int& hd, int& n, int& 
 // res writes (made visible to thread 0 by the barrier) before the count, so a host that reads t with acquire semantics
 // reads their results too.  The fence waits for the pass's res writes to reach host memory, ~3 us on H100 (config 2: the
 // candidate phase grew by 6.5 k SM clocks per pass when every pass published), so it is paid once per 8 passes.
-LT_FN void publish(const Args& a, int t) {
+// A speculative launch also reads its abort word here into s.stop, which every thread reads at the end of the same pass, so
+// the whole block leaves together.
+LT_FN void publish(const Args& a, Shared& s, int t) {
 #if LT_DEV
-    if (a.prog && threadIdx.x == 0) { __threadfence_system(); *a.prog = t; }
+    if (threadIdx.x == 0) {
+        if (a.prog) { __threadfence_system(); *a.prog = t; }
+        if (a.abort) s.stop = *a.abort;
+    }
 #else
-    (void)a; (void)t;
+    (void)a; (void)s; (void)t;
 #endif
 }
 
 // ---- the stretch -------------------------------------------------------------------------------------------------
 template <int D>
 LT_FN void stretch(const Args& a, Shared& s) {
-    const int RS = a.RS, nlive = a.nlive, B = a.B;
+    const int RS = a.RS, nlive = a.nlive;
+    // (every thread reads the same words: the whole block returns, or none of it)
+    if (a.go && (a.go[ykspec::W_STATUS] != ykspec::GO || *a.nan)) {
+        LT_ONE { a.hdr[R_CONSUMED] = 0; a.hdr[R_STATUS] = ST_ABORTED; a.hdr[R_PASSES] = 0; a.hdr[R_SINGLES] = 0; a.hdr[R_SPENT] = 0; }
+        return;
+    }
     int buf = *a.cur;
     int t = 0, status = yklt::ST_DONE, passes = 0, singles = 0;
 #if LT_DEV
@@ -310,12 +329,13 @@ LT_FN void stretch(const Args& a, Shared& s) {
 
     // ---- the stretch's requests staged in stretch order, and the smallest per dimension (requests of an ask that
     // reaches a commit are >= 0) ----
-    LT_ONE { for (int k = 0; k < 8; ++k) s.minreq[k] = INT64_MAX; s.n_sp = 0; s.keep = 0; s.nan = 0; }
+    // (the stretch's length is read from s.B where it is used: held in a register through every round, it spills)
+    LT_ONE { for (int k = 0; k < 8; ++k) s.minreq[k] = INT64_MAX; s.n_sp = 0; s.keep = 0; s.nan = 0; s.stop = 0; s.B = a.go ? (int)a.go[ykspec::W_COUNT] : a.B; }
     LT_SYNC();
     {
         u64 my[D];
         for (int k = 0; k < D; ++k) my[k] = KEY_INF;
-        LT_FOR(i, B) {
+        LT_FOR(i, s.B) {
             const uint32_t ask = a.asks[i];
             for (int k = 0; k < D; ++k) {
                 const int64_t v = a.a_req[(size_t)k * a.lda + ask];
@@ -357,9 +377,9 @@ LT_FN void stretch(const Args& a, Shared& s) {
     int hd = 0, nl = 0, lb = 0;
     LT_PROF(RP_EDGES);
 
-    while (t < B) {
-        if ((passes & (PUBLISH_PASSES - 1)) == 0) publish(a, t);   // (the res writes so far are behind the barriers that ended their passes)
-        const int left = B - t;
+    while (t < s.B) {
+        if ((passes & (PUBLISH_PASSES - 1)) == 0) publish(a, s, t);   // (the res writes so far are behind the barriers that ended their passes)
+        const int left = s.B - t;
         int W = a.window < left ? a.window : left;
         W = W < n_act + nl ? W : n_act + nl;
         const int wm = W < n_act ? W : n_act, wl = W < nl ? W : nl;
@@ -504,7 +524,10 @@ LT_FN void stretch(const Args& a, Shared& s) {
             LT_PROF(RP_SINGLE);
         }
         if (moved) buf ^= 1;
-        if (a.guard > 0 && passes >= GUARD_PASSES && t < B && (long long)t < (long long)a.guard * passes) {
+        // a publishing pass reads s.stop after its last barrier; thread 0 writes it next at the top of the next publishing
+        // pass, behind the barriers of the passes between
+        if (((passes - 1) & (PUBLISH_PASSES - 1)) == 0 && s.stop) { status = ST_ABORTED; break; }
+        if (a.guard > 0 && passes >= GUARD_PASSES && t < s.B && (long long)t < (long long)a.guard * passes) {
             status = yklt::ST_HANDOFF;
             break;
         }

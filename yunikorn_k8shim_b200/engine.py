@@ -57,7 +57,8 @@ class Stats(C.Structure):
                 ("lattice_cycles", C.c_uint64),
                 ("uniform_runs", C.c_uint64), ("uniform_asks", C.c_uint64), ("uniform_elements", C.c_uint64),
                 ("uniform_retries", C.c_uint64),
-                ("round_passes", C.c_uint64), ("round_asks", C.c_uint64), ("round_single_steps", C.c_uint64)]
+                ("round_passes", C.c_uint64), ("round_asks", C.c_uint64), ("round_single_steps", C.c_uint64),
+                ("spec_adopted", C.c_uint64), ("spec_discarded", C.c_uint64)]
 
     def as_dict(self):
         d = {f: getattr(self, f) for f, _ in self._fields_}

@@ -85,6 +85,9 @@ type askRec struct {
 	slow      bool
 	exact     bool // slow only for needsGoPredicates: the dictionary encoded the pod's masks exactly (yk_filter_nodes applies)
 	present   bool
+	ppFlags   C.uint32_t // YK_ASK_NO_PREEMPT_SELF / _OTHER / YK_ASK_ORIGINATOR from the ask's PreemptionPolicy and Originator
+	blocked   time.Time  // when the ask was first reported NOFIT / SKIPPED since it last was anything else (zero: not blocked)
+	pinNode   uint32     // none, or the node a preemption plan holds for it: written as its required node
 }
 
 type Engine struct {
@@ -106,6 +109,7 @@ type Engine struct {
 	appQueue []uint32
 	queueIdx map[string]uint32 // "root.a.b" -> index
 	queueLeaf []bool
+	queueDelay []time.Duration // preemption.delay per queue: how long a blocked ask waits before it may preempt
 	nodeSort nodeSort // what yk_node_sort_set last applied: put back when the rest of a configuration is refused
 	seq      int64
 	stop     chan struct{}
@@ -280,7 +284,8 @@ func (e *Engine) setQueues(root []queueConf) error {
 	var guar, max [][4]int64
 	var sortPol []C.uint8_t
 	var off []C.int32_t
-	var fence []C.uint8_t
+	var fence, ppFence []C.uint8_t
+	var delay []time.Duration
 	idx := map[string]uint32{}
 	var leaf []bool
 	var walk func(q queueConf, p uint32, path string)
@@ -300,6 +305,16 @@ func (e *Engine) setQueues(root []queueConf) error {
 			f = 1
 		}
 		fence = append(fence, f)
+		pf := C.uint8_t(0)
+		if q.Properties["preemption.policy"] == "fence" {
+			pf = 1
+		}
+		ppFence = append(ppFence, pf)
+		d, err := time.ParseDuration(q.Properties["preemption.delay"])
+		if err != nil || d <= 0 {
+			d = 30 * time.Second // the core's default
+		}
+		delay = append(delay, d)
 		idx[path] = me
 		leaf = append(leaf, len(q.Queues) == 0 && !q.Parent)
 		for _, c := range q.Queues {
@@ -323,7 +338,10 @@ func (e *Engine) setQueues(root []queueConf) error {
 	if err := e.ck(C.yk_queues_priority(e.h, C.uint32_t(n), &off[0], &fence[0]), "yk_queues_priority"); err != nil {
 		return err
 	}
-	e.queueIdx, e.queueLeaf = idx, leaf
+	if err := e.ck(C.yk_queues_preemption(e.h, C.uint32_t(n), &ppFence[0]), "yk_queues_preemption"); err != nil {
+		return err
+	}
+	e.queueIdx, e.queueLeaf, e.queueDelay = idx, leaf, delay
 	return nil
 }
 
@@ -821,10 +839,25 @@ func (e *Engine) pushAsk(idx uint32, a *askRec, alloc *si.Allocation) error {
 		e.seq++
 		a.prio, a.seq = alloc.Priority, created<<20|e.seq&0xFFFFF // seconds tie: break by arrival (SURVEY A.6)
 		a.lastState = C.YK_ST_PENDING
+		a.ppFlags, a.pinNode = 0, none
+		if pp := alloc.PreemptionPolicy; pp != nil {
+			if !pp.AllowPreemptSelf {
+				a.ppFlags |= C.YK_ASK_NO_PREEMPT_SELF
+			}
+			if !pp.AllowPreemptOther {
+				a.ppFlags |= C.YK_ASK_NO_PREEMPT_OTHER
+			}
+		}
+		if alloc.Originator {
+			a.ppFlags |= C.YK_ASK_ORIGINATOR
+		}
 	}
 	prio, seq := C.int32_t(a.prio), C.int64_t(a.seq)
 	i, capp := C.uint32_t(idx), C.uint32_t(app)
-	tol, need, deny, rn, fl := m.tolerated_bits, m.required_bits, m.forbidden_bits, m.required_node, m.flags
+	tol, need, deny, rn, fl := m.tolerated_bits, m.required_bits, m.forbidden_bits, m.required_node, m.flags|a.ppFlags
+	if a.pinNode != none {
+		rn = C.uint32_t(a.pinNode)
+	}
 	return e.ck(C.yk_asks_upsert(e.h, 1, &i, &rq[0], &tol, &need, &deny, &prio, &seq, &capp, &rn, &fl, nil), "yk_asks_upsert")
 }
 
@@ -985,8 +1018,10 @@ func (e *Engine) loop() {
 				ResourcePerAlloc: nil /* the shim only reads key, application and node: scheduler_callback.go:53-76 */})
 		}
 		var states []*si.UpdateContainerSchedulingStateRequest
+		var preempted *si.AllocationResponse
 		if rc == C.YK_OK {
 			states = e.collectStates()
+			preempted = e.preempt()
 		}
 		slowKeys := make([]uint32, 0, int(nslow))
 		for i := 0; i < int(nslow); i++ {
@@ -1007,8 +1042,70 @@ func (e *Engine) loop() {
 		for _, s := range states {
 			cb.UpdateContainerSchedulingState(s)
 		}
+		if preempted != nil {
+			_ = cb.UpdateAllocation(preempted) // -> ForgetPod + the task's release event (scheduler_callback.go:102-115)
+		}
 		e.slowPath(cb, slowKeys)
 	}
+}
+
+// preempt: the core's preemption for queues below their guarantee, once per loop, for the asks blocked (NOFIT / SKIPPED)
+// for at least their queue's preemption.delay, oldest first (yk_preemption_plan, DESIGN.md §2 item 9).  A plan's victims are
+// released here and handed to the shim as preempted; the preemptor is pinned to the planned node through its required node,
+// so the next cycle places it there.  Called with e.mu held; nil when nothing was preempted.
+func (e *Engine) preempt() *si.AllocationResponse {
+	now := time.Now()
+	var asks []C.uint32_t
+	for i := range e.asks {
+		a := &e.asks[i]
+		if !a.present || a.foreign || a.slow || a.blocked.IsZero() || a.pinNode != none {
+			continue
+		}
+		d := 30 * time.Second
+		if q := e.appQueue[e.appIdx[a.app]]; int(q) < len(e.queueDelay) {
+			d = e.queueDelay[q]
+		}
+		if now.Sub(a.blocked) >= d {
+			asks = append(asks, C.uint32_t(i))
+		}
+	}
+	if len(asks) == 0 {
+		return nil
+	}
+	sort.Slice(asks, func(x, y int) bool { return e.asks[asks[x]].blocked.Before(e.asks[asks[y]].blocked) })
+	n := len(asks)
+	status, node := make([]C.uint32_t, n), make([]C.uint32_t, n)
+	off, victims := make([]C.uint32_t, n+1), make([]C.uint32_t, len(e.asks)+1)
+	var done C.uint32_t
+	if e.ck(C.yk_preemption_plan(e.h, C.uint32_t(n), &asks[0], &status[0], &node[0], &off[0], &victims[0],
+		C.uint32_t(len(victims)), &done), "yk_preemption_plan") != nil {
+		return nil
+	}
+	resp := &si.AllocationResponse{}
+	for j := 0; j < int(done); j++ {
+		if status[j] != C.YK_PP_PLANNED {
+			continue
+		}
+		vs := victims[off[j]:off[j+1]]
+		if C.yk_release(e.h, C.uint32_t(len(vs)), &vs[0]) != C.YK_OK {
+			continue
+		}
+		for _, v := range vs {
+			a := &e.asks[v]
+			resp.Released = append(resp.Released, &si.AllocationRelease{ApplicationID: a.app, AllocationKey: a.key,
+				TerminationType: si.TerminationType_PREEMPTED_BY_SCHEDULER, Message: "preempted by scheduler"})
+			a.present = false
+			delete(e.askIdx, a.key)
+			e.freeAsks = append(e.freeAsks, uint32(v))
+		}
+		p := &e.asks[asks[j]]
+		p.pinNode = uint32(node[j])
+		_ = e.pushAsk(uint32(asks[j]), p, nil)
+	}
+	if len(resp.Released) == 0 {
+		return nil
+	}
+	return resp
 }
 
 // collectStates: asks that ended the cycle NOFIT / SKIPPED and were not reported in that state yet ->
@@ -1050,6 +1147,13 @@ func (e *Engine) collectStates() []*si.UpdateContainerSchedulingStateRequest {
 		s := uint8(st[j])
 		if s == a.lastState {
 			continue
+		}
+		if s == C.YK_ST_NOFIT || s == C.YK_ST_SKIPPED {
+			if a.lastState != C.YK_ST_NOFIT && a.lastState != C.YK_ST_SKIPPED {
+				a.blocked = time.Now()
+			}
+		} else {
+			a.blocked = time.Time{}
 		}
 		a.lastState = s
 		switch s {

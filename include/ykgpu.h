@@ -39,6 +39,7 @@
  *   yk_preemption_search                ResourceManagerCallback.PreemptionPredicates for one (ask, node, victims) query
  *   yk_preemption_nodes                 the same search on every node for a list of asks, from the allocations the
  *                                       engine made: the search half of a preemptor (its policy stays with the caller)
+ *   yk_preemption_plan                  the core's preemption for queues below their guarantee: victims, node and marks
  *
  * Conventions: every call returns YK_OK (0) or a negative yk_status; no exceptions or aborts cross the
  * boundary.  Inputs are caller-owned host memory, fully consumed before return (cgo: no Go pointer is
@@ -83,6 +84,11 @@ typedef enum {
 #define YK_ASK_SLOWPATH 1u       /* carries a predicate that does not reduce to the masks (ports, volumes,
                                     pod (anti-)affinity, topology spread): never bound by yk_cycle, returned
                                     in its slow-path list for the unchanged Go PredicateManager */
+/* preemption policy of the pod (si.PreemptionPolicy, pkg/cache/task.go:233-258): read only by yk_preemption_plan, never by
+   yk_cycle (they are not part of the sweep's row signature) */
+#define YK_ASK_NO_PREEMPT_SELF 2u   /* not AllowPreemptSelf: taken as a victim only after every allocation without it */
+#define YK_ASK_NO_PREEMPT_OTHER 4u  /* not AllowPreemptOther (preemptionPolicy: Never): never preempts */
+#define YK_ASK_ORIGINATOR 8u        /* the pod that originated its application: taken as a victim after the others */
 /* per-ask state reported by yk_ask_states */
 #define YK_ST_PENDING 0u
 #define YK_ST_ALLOCATED 1u
@@ -204,6 +210,11 @@ int yk_queues_set(yk_engine* e, uint32_t q, const uint32_t* parent, const int64_
  * Both arrays are [q] in yk_queues_set order and may be NULL (= 0 / no fence); yk_queues_set resets them.  Behaviour
  * checked by the reference in test/e2e/priority_scheduling/priority_scheduling_test.go:70-251. */
 int yk_queues_priority(yk_engine* e, uint32_t q, const int32_t* offset, const uint8_t* fence);
+
+/* optional queue property preemption.policy of the core's queue configuration: fence[i] != 0 = "fence" (a preemptor below queue
+ * i takes victims only inside i's subtree).  [q] in yk_queues_set order, NULL = no fence; yk_queues_set resets it.  Read only by
+ * yk_preemption_plan. */
+int yk_queues_preemption(yk_engine* e, uint32_t q, const uint8_t* fence);
 
 /* applications live in LEAF queues (as in the core: placement into a parent queue is rejected there; here an application
  * whose queue has children is accepted but never scheduled -- the adapter must not produce one) */
@@ -368,6 +379,54 @@ int yk_preemption_nodes(yk_engine* e, uint32_t n, const uint32_t* asks,
                         uint32_t* need_out /* [n][k] victims needed on that node, 0 padded; may be NULL */,
                         uint32_t* n_fit /* [n], may be NULL */,
                         uint32_t* best_node /* [n], may be NULL */, uint32_t* best_need /* [n], may be NULL */);
+
+/* Preemption for queues below their guarantee: for each preemptor, in the order given, the victims and the node that let it run
+ * (the core's guarantee preemption, DESIGN.md §2 item 9), evaluated on the device (csrc/yk_preempt_plan.cuh).  A plan MARKS
+ * its victims and records the preemptor as planned on its node; the caller releases the victims (yk_release) and pins the
+ * preemptor (required_node), and the next yk_cycle places it.  yk_cycle never reads marks or plans.
+ *   For plan calls, usage(q) = allocated(q) - marked victims below q + requests of planned preemptors below q, and
+ *   room(node) = available + marked victims on it - requests of planned preemptors on it.  Later preemptors of one call see the
+ *   marks and plans of the earlier ones.
+ *   Status per ask (status_out[i]):
+ *     YK_PP_NOT_BLOCKED  not present, state not YK_ST_NOFIT / YK_ST_SKIPPED, or already planned by an earlier call;
+ *     YK_PP_NOT_ALLOWED  YK_ASK_NO_PREEMPT_OTHER, or over the headroom of a user limit that applies to it;
+ *     YK_PP_UNSUPPORTED  slow path, gang member or required node;
+ *     YK_PP_GUARANTEE    its leaf has no guarantee, or some queue on its path with a guarantee would go over it;
+ *     YK_PP_NO_VICTIMS   no node fits it with victims, or the queue headroom cannot be freed;
+ *     YK_PP_FITS         a node fits it and no victim is needed (the next cycle places it): nothing is marked;
+ *     YK_PP_PLANNED      victims marked, the ask planned on node_out[i].
+ *   Victims: an allocation bound by this engine to a present node, not marked, without a required node, outside the
+ *     preemptor's leaf, inside the fence root's subtree (the nearest queue on the preemptor's path with preemption fence, or
+ *     root), whose priority plus the priority.offset of its queues strictly below the lowest common ancestor is at most the
+ *     preemptor's computed the same way.  Order: without YK_ASK_NO_PREEMPT_SELF first, non-originators first, adjusted
+ *     priority ascending (saturated to int32), create_seq descending, index.  A victim is taken only if every queue with a
+ *     guarantee on its path strictly below the lowest common ancestor stays at or above it with every victim taken so far.
+ *   Node: of the present nodes that pass the preemptor's static steps (schedulable, taints, labels, total), the one needing the
+ *     fewest of its own victims (in order) until request <= max(0, room); ties to the earlier node in the cycle's order.
+ *   Headroom: while a queue on the preemptor's path with a max is over it (usage + request > max), further victims in order from
+ *     any node below a queue still over its max are taken; if they run out the status is YK_PP_NO_VICTIMS and nothing is marked.
+ *   Output: node_out[i] = the node (PLANNED / FITS) or YK_NONE; the victims of ask i are
+ *     victims_out[victim_off_out[i] .. victim_off_out[i+1]), node victims first, each group in victim order.  Planning stops
+ *     before the first ask whose victims would pass victims_cap; *n_done = the asks handled, and only status_out / node_out
+ *     [0, n_done) and victim_off_out [0, n_done] are written.
+ *   Marks clear when the allocation is released (yk_release); plans when the preemptor is allocated by a cycle, removed,
+ *     upserted again or resized.
+ *   Errors, all checked before anything is marked; nothing changes on an error:
+ *     YK_ERR_ARG   asks / status_out / node_out / victim_off_out / n_done NULL with n > 0, victims_out NULL with victims_cap > 0,
+ *                  an index >= max_asks, the same ask twice;
+ *     YK_ERR_RANGE a present node scores NaN (as yk_cycle).
+ *   A YK_ERR_CUDA rolls every mark and plan of the call back.  n == 0 is YK_OK.  Counted in other_launches / h2d_bytes /
+ *   d2h_bytes.  Multi-GPU split sweep (world > 1): every rank makes the same call between the same two cycles. */
+#define YK_PP_PLANNED 0u
+#define YK_PP_FITS 1u
+#define YK_PP_NOT_BLOCKED 2u
+#define YK_PP_NOT_ALLOWED 3u
+#define YK_PP_UNSUPPORTED 4u
+#define YK_PP_GUARANTEE 5u
+#define YK_PP_NO_VICTIMS 6u
+int yk_preemption_plan(yk_engine* e, uint32_t n, const uint32_t* asks, uint32_t* status_out, uint32_t* node_out,
+                       uint32_t* victim_off_out /* [n+1] */, uint32_t* victims_out /* [victims_cap] */, uint32_t victims_cap,
+                       uint32_t* n_done);
 
 /* multi-GPU exchange hook: called once per batch on every rank, after the local shard's rows of `buf`
  * (device pointer, row-major, `row_bytes` per ask, rows [first_row, first_row+n_rows) are this rank's)

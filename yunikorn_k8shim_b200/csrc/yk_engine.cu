@@ -31,6 +31,7 @@
 #include "yk_kernels.cuh"
 #include "yk_filter.cuh"
 #include "yk_preempt_nodes.cuh"
+#include "yk_preempt_plan.cuh"
 #include "yk_lattice.cuh"
 #include "yk_uniform.cuh"
 #include "yk_rounds.cuh"
@@ -322,6 +323,12 @@ struct yk_engine {
     Dev<uint64_t> pn_key_in, pn_key_out; Dev<int64_t> pn_vreq; Dev<int32_t> pn_res; Dev<uint8_t> pn_cub;
     Pin<uint32_t> h_pn_in, h_pn_out;
     std::vector<uint32_t> pn_seen; uint32_t pn_stamp = 0;
+    // yk_preemption_plan: the queues' preemption fence, the marked victims and each planned preemptor's node (YK_NONE: none);
+    // per-call device tables (queues, bound allocations, room), per-preemptor sort buffers and results, grown on demand
+    std::vector<uint8_t> q_pp_fence, pp_mark; std::vector<uint32_t> pp_plan;
+    Dev<uint32_t> pp_q32, pp_v32, pp_tv[2], pp_nkey[2], pp_nval[2], pp_seg, pp_cnt, pp_pnode; Dev<int32_t> pp_vprio;
+    Dev<int64_t> pp_q64, pp_room, pp_pval; Dev<uint64_t> pp_key[2]; Dev<unsigned long long> pp_best;
+    Dev<uint8_t> pp_hasg, pp_taken, pp_cub;
     yk_allgather_fn xfn = nullptr; void* xctx = nullptr;
     // peer-to-peer exchange (see yk_peer_export): peers' slot buffers and sync blocks, mapped through CUDA IPC
     bool p2p = false;
@@ -1508,6 +1515,7 @@ int yk_create(const yk_config* cfg, yk_engine** out) {
     e->sigs.reset(A);
     e->a_sig.assign(A, 0); e->a_prio.assign(A, 0); e->a_create.assign(A, 0); e->a_app.assign(A, 0); e->a_flags.assign(A, 0);
     e->a_gang.assign(A, YK_NONE); e->a_bound.assign(A, YK_NONE); e->a_state.assign(A, yk::ST_ABSENT);
+    e->pp_mark.assign(A, 0); e->pp_plan.assign(A, YK_NONE);
     e->p_queue.assign(e->maxP, 0); e->p_submit.assign(e->maxP, 0); e->p_present.assign(e->maxP, 0); e->p_user.assign(e->maxP, YK_NONE);
     e->p_alloc.assign((size_t)e->maxP * D, 0);
     // default queue tree: root only would have no leaf for apps; root + one leaf "root.default"
@@ -1600,6 +1608,7 @@ int yk_queues_set(yk_engine* e, uint32_t q, const uint32_t* parent, const int64_
     e->q_sort.assign(q, 0);
     if (sort) e->q_sort.assign(sort, sort + q);
     e->q_prio_offset.assign(q, 0); e->q_prio_fence.assign(q, 0);   // defaults; yk_queues_priority sets them
+    e->q_pp_fence.assign(q, 0);                                      // yk_queues_preemption sets it
     for (uint32_t i = 0; i < q; ++i)
         if (e->q_sort[i] > 1) return e->fail(YK_ERR_ARG, "yk_queues_set: unknown application sort policy");
     return YK_OK;
@@ -1612,6 +1621,15 @@ int yk_queues_priority(yk_engine* e, uint32_t q, const int32_t* offset, const ui
     e->q_prio_offset.assign(q, 0); e->q_prio_fence.assign(q, 0);
     if (offset) e->q_prio_offset.assign(offset, offset + q);
     if (fence) for (uint32_t i = 0; i < q; ++i) e->q_prio_fence[i] = fence[i] ? 1 : 0;
+    return YK_OK;
+}
+
+int yk_queues_preemption(yk_engine* e, uint32_t q, const uint8_t* fence) {
+    if (!e) return YK_ERR_ARG;
+    std::lock_guard<std::mutex> g(e->mu);
+    if (q != e->nq) return e->fail(YK_ERR_ARG, "yk_queues_preemption: queue count differs from yk_queues_set");
+    e->q_pp_fence.assign(q, 0);
+    if (fence) for (uint32_t i = 0; i < q; ++i) e->q_pp_fence[i] = fence[i] ? 1 : 0;
     return YK_OK;
 }
 
@@ -1678,6 +1696,7 @@ int yk_asks_upsert(yk_engine* e, uint32_t a, const uint32_t* idx, const int64_t*
             return e->fail(YK_ERR_ARG, "yk_asks_upsert: required_node beyond max_nodes");
         if (e->a_state[idx[i]] == yk::ST_ALLOCATED) return e->fail(YK_ERR_STATE, "yk_asks_upsert: ask holds an allocation (release it first)");
     }
+    for (uint32_t i = 0; i < a; ++i) e->pp_plan[idx[i]] = YK_NONE;   // a new ask: an earlier plan for the index is gone
     const yk::CommitTables sv = sig_view(e);
     if (contiguous_run(idx, a)) {   // whole-column copies, then the signature hashes in one sequential pass
         const uint32_t x0 = idx[0];
@@ -1738,7 +1757,7 @@ int yk_asks_remove(yk_engine* e, uint32_t a, const uint32_t* idx) {
         if (idx[i] >= e->maxA) return e->fail(YK_ERR_ARG, "yk_asks_remove: index beyond max_asks");
         if (e->a_state[idx[i]] == yk::ST_ALLOCATED) return e->fail(YK_ERR_STATE, "yk_asks_remove: ask holds an allocation (use yk_release)");
     }
-    for (uint32_t i = 0; i < a; ++i) e->a_state[idx[i]] = yk::ST_ABSENT;
+    for (uint32_t i = 0; i < a; ++i) { e->a_state[idx[i]] = yk::ST_ABSENT; e->pp_plan[idx[i]] = YK_NONE; }
     return YK_OK;
 }
 
@@ -1756,6 +1775,7 @@ int yk_release(yk_engine* e, uint32_t n, const uint32_t* idx) {
         alloc_move(e, a, d);
         e->a_state[a] = yk::ST_ABSENT;
         e->a_bound[a] = YK_NONE;
+        e->pp_mark[a] = 0;
     }
     e->nodes_stale = true;
     return YK_OK;
@@ -1807,6 +1827,7 @@ int yk_asks_resize(yk_engine* e, uint32_t n, const uint32_t* idx, const int64_t*
             r = req[(size_t)k * n + i];
         }
         if (!same) ask_resign(e, sv, x);
+        e->pp_plan[x] = YK_NONE;
     }
     if (n) e->nodes_stale = e->asks_stale = true;
     return YK_OK;
@@ -2517,6 +2538,352 @@ int yk_preemption_nodes(yk_engine* e, uint32_t n, const uint32_t* asks, const ui
         }
         c0 = c1;
     }
+    return YK_OK;
+}
+
+// Rules 1-2 and 7-8 of the plan run here on the host; rules 3-6 (every bound allocation, every node) on the device.  The host
+// repeats rule 5 only on the chosen node's segment and on the headroom step's list, both read back in victim order.
+int yk_preemption_plan(yk_engine* e, uint32_t n, const uint32_t* asks, uint32_t* status_out, uint32_t* node_out,
+                       uint32_t* victim_off_out, uint32_t* victims_out, uint32_t victims_cap, uint32_t* n_done) {
+    if (!e) return YK_ERR_ARG;
+    std::lock_guard<std::mutex> g(e->mu);
+    if (n && (!asks || !status_out || !node_out || !victim_off_out || !n_done))
+        return e->fail(YK_ERR_ARG, "yk_preemption_plan: null asks, status_out, node_out, victim_off_out or n_done");
+    if (victims_cap && !victims_out) return e->fail(YK_ERR_ARG, "yk_preemption_plan: null victims_out with victims_cap > 0");
+    if (!n) { if (n_done) *n_done = 0; if (victim_off_out) victim_off_out[0] = 0; return YK_OK; }
+    if (e->pn_seen.size() < e->maxA) { e->pn_seen.assign(e->maxA, 0); e->pn_stamp = 0; }
+    if (++e->pn_stamp == 0) { std::fill(e->pn_seen.begin(), e->pn_seen.end(), 0u); e->pn_stamp = 1; }
+    for (uint32_t i = 0; i < n; ++i) {
+        if (asks[i] >= e->maxA) return e->fail(YK_ERR_ARG, "yk_preemption_plan: ask index beyond max_asks");
+        if (e->pn_seen[asks[i]] == e->pn_stamp) return e->fail(YK_ERR_ARG, "yk_preemption_plan: the same ask twice");
+        e->pn_seen[asks[i]] = e->pn_stamp;
+    }
+    int rc = upload_tables(e);
+    if (rc) return rc;
+    const int D = e->D;
+    const uint32_t nlive = e->nlive, nq = e->nq, A = e->a_hi, N = e->maxN;
+    cudaStream_t s = e->stream;
+    std::vector<uint32_t> order(nlive);
+    if (nlive) {   // the cycle's node order, and the NaN check before anything is marked
+        CK(grow(e->pn_pos, e->maxN));
+        rc = filter_order(e, e->cfg.policy, e->w);
+        if (rc) return rc;
+        yk_pn_pos_kernel<<<(nlive + 255) / 256, 256, 0, s>>>(e->f_val_out.p, (int)nlive, e->pn_pos.p);
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(order.data(), e->f_val_out.p, 4 * (size_t)nlive, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        e->st.other_launches += 1;
+        e->st.d2h_bytes += 4 * (size_t)nlive;
+        if (e->h_f_flag[0]) return e->fail(YK_ERR_RANGE, "yk_preemption_plan: NaN node score (zero total on a weighted resource)");
+    }
+    // a plan whose preemptor a cycle has since allocated is spent
+    for (uint32_t a = 0; a < A; ++a) if (e->pp_plan[a] != YK_NONE && e->a_state[a] == yk::ST_ALLOCATED) e->pp_plan[a] = YK_NONE;
+    const std::vector<uint8_t> mark0 = e->pp_mark;
+    const std::vector<uint32_t> plan0 = e->pp_plan;
+    auto bail = [&](int code) { e->pp_mark = mark0; e->pp_plan = plan0; return code; };
+#define PK(call)                                                                   \
+    do {                                                                           \
+        cudaError_t _e = (call);                                                   \
+        if (_e != cudaSuccess) return bail(e->cuda_fail(_e, #call));               \
+    } while (0)
+
+    // ---- queue tables: depth, preorder interval, prefix offsets, guarantee flag, usage for plan calls ----
+    const uint32_t* par = e->q_parent.data();
+    std::vector<uint32_t> q32(4 * (size_t)nq);   // parent, depth, tin, tout
+    uint32_t* depth = q32.data() + nq; uint32_t* tin = depth + nq; uint32_t* tout = tin + nq;
+    std::vector<int64_t> q64((size_t)nq * (1 + 2 * D), 0);   // poff, guar, use
+    int64_t* poff = q64.data(); int64_t* guar = poff + nq; int64_t* use = guar + (size_t)D * nq;
+    std::vector<uint8_t> hasg(nq, 0);
+    {
+        std::vector<std::vector<uint32_t>> kids(nq);
+        for (uint32_t q = 1; q < nq; ++q) kids[par[q]].push_back(q);
+        std::vector<std::pair<uint32_t, size_t>> st{{0u, 0}};
+        uint32_t clock = 0;
+        tin[0] = clock++;
+        while (!st.empty()) {   // preorder: q is an ancestor-or-self of x iff tin[q] <= tin[x] < tout[q]
+            auto& [q, c] = st.back();
+            if (c < kids[q].size()) { const uint32_t ch = kids[q][c++]; tin[ch] = clock++; st.push_back({ch, 0}); }
+            else { tout[q] = clock; st.pop_back(); }
+        }
+    }
+    for (uint32_t q = 0; q < nq; ++q) {
+        q32[q] = par[q];
+        depth[q] = q ? depth[par[q]] + 1 : 0;
+        poff[q] = (q ? poff[par[q]] : 0) + e->q_prio_offset[q];
+        for (int k = 0; k < D; ++k) {
+            guar[(size_t)k * nq + q] = e->q_guar[(size_t)k * nq + q];
+            use[(size_t)k * nq + q] = e->q_alloc[(size_t)k * nq + q];
+            if (guar[(size_t)k * nq + q] >= 0) hasg[q] = 1;
+        }
+    }
+    auto leaf_of = [&](uint32_t a) { return e->p_queue[e->a_app[a]]; };
+    auto req = [&](uint32_t a, int k) { return e->a_req[(size_t)k * e->maxA + a]; };
+    auto chain_add = [&](uint32_t a, int sign) {
+        for (uint32_t q = leaf_of(a); q != YK_NONE; q = par[q])
+            for (int k = 0; k < D; ++k) use[(size_t)k * nq + q] += sign * req(a, k);
+    };
+    // room for plan calls, and the bound allocations (slots) in ask-index order
+    std::vector<int64_t> room((size_t)D * N, 0);
+    for (uint32_t x = 0; x < e->n_hi; ++x)
+        if (e->n_present[x]) for (int k = 0; k < D; ++k) room[(size_t)k * N + x] = e->n_avail[(size_t)k * N + x];
+    std::vector<uint32_t> slot_of(A, YK_NONE), v32, vask, vleaf, vflag, vnode; std::vector<int32_t> vprio; std::vector<uint64_t> ckey;
+    for (uint32_t a = 0; a < A; ++a) {
+        if (e->pp_mark[a] && e->a_state[a] == yk::ST_ALLOCATED) {
+            chain_add(a, -1);
+            const uint32_t x = e->a_bound[a];
+            if (x < N && e->n_present[x]) for (int k = 0; k < D; ++k) room[(size_t)k * N + x] += req(a, k);
+        }
+        if (e->pp_plan[a] != YK_NONE && e->a_state[a] != yk::ST_ABSENT) {
+            chain_add(a, +1);
+            const uint32_t x = e->pp_plan[a];
+            if (e->n_present[x]) for (int k = 0; k < D; ++k) room[(size_t)k * N + x] -= req(a, k);
+        }
+        const uint32_t x = e->a_bound[a];
+        if (e->a_state[a] != yk::ST_ALLOCATED || x >= N || !e->n_present[x]) continue;
+        slot_of[a] = (uint32_t)vask.size();
+        vask.push_back(a); vleaf.push_back(leaf_of(a)); vnode.push_back(x); vprio.push_back(e->a_prio[a]);
+        const uint32_t f = e->a_flags[a];
+        vflag.push_back(((f & YK_ASK_NO_PREEMPT_SELF) ? YK_PPF_NO_SELF : 0u) | ((f & YK_ASK_ORIGINATOR) ? YK_PPF_ORIGINATOR : 0u) |
+                        ((e->a_node[a] != YK_NONE || e->pp_mark[a]) ? YK_PPF_OUT : 0u));
+        ckey.push_back(~((uint64_t)e->a_create[a] ^ (1ull << 63)));   // ascending key = create_seq descending
+    }
+    const uint32_t m = (uint32_t)vask.size();
+    if (m >= (1u << 30)) return bail(e->fail(YK_ERR_RANGE, "yk_preemption_plan: 2^30 or more bound allocations"));
+
+    // ---- device tables of the call ----
+    const auto bits = [](uint32_t x) { return x ? 32 - __builtin_clz(x) : 0; };
+    const int nbits = std::max(1, bits(nlive));   // node keys 0 .. nlive (nlive = not eligible)
+    const size_t M = std::max<uint32_t>(m, 1);
+    PK(grow(e->pp_q32, q32.size())); PK(grow(e->pp_q64, q64.size())); PK(grow(e->pp_hasg, nq));
+    PK(grow(e->pp_v32, 5 * M)); PK(grow(e->pp_vprio, M)); PK(grow(e->pp_taken, M));
+    for (int b = 0; b < 2; ++b) { PK(grow(e->pp_key[b], M)); PK(grow(e->pp_tv[b], M)); PK(grow(e->pp_nkey[b], M)); PK(grow(e->pp_nval[b], M)); }
+    PK(grow(e->pp_seg, 2 * (size_t)std::max<uint32_t>(nlive, 1))); PK(grow(e->pp_cnt, 1)); PK(grow(e->pp_best, 1));
+    PK(grow(e->pp_room, (size_t)D * N)); PK(grow(e->pp_pnode, M + 1)); PK(grow(e->pp_pval, (size_t)D * (M + 1)));
+    size_t b1 = 0, b2 = 0;
+    PK(cub::DeviceRadixSort::SortPairs(nullptr, b1, e->pp_key[0].p, e->pp_key[1].p, e->pp_tv[0].p, e->pp_tv[1].p, (int)M, 0, 64, s));
+    PK(cub::DeviceRadixSort::SortPairs(nullptr, b2, e->pp_nkey[0].p, e->pp_nkey[1].p, e->pp_nval[0].p, e->pp_nval[1].p, (int)M, 0, nbits, s));
+    PK(grow(e->pp_cub, std::max(b1, b2)));
+    uint32_t* d_ask = e->pp_v32.p; uint32_t* d_leaf = d_ask + M; uint32_t* d_flag = d_leaf + M; uint32_t* d_node = d_flag + M;
+    uint32_t* d_perm = d_node + M;
+    PK(cudaMemcpyAsync(e->pp_q32.p, q32.data(), 4 * q32.size(), cudaMemcpyHostToDevice, s));
+    PK(cudaMemcpyAsync(e->pp_q64.p, q64.data(), 8 * (size_t)nq * (1 + D), cudaMemcpyHostToDevice, s));   // poff, guar
+    PK(cudaMemcpyAsync(e->pp_hasg.p, hasg.data(), nq, cudaMemcpyHostToDevice, s));
+    PK(cudaMemcpyAsync(e->pp_room.p, room.data(), 8 * room.size(), cudaMemcpyHostToDevice, s));
+    e->st.h2d_bytes += 4 * q32.size() + 8 * (size_t)nq * (1 + D) + nq + 8 * room.size();
+    std::vector<uint32_t> perm(m);
+    if (m) {   // the create-order positions: one stable sort of the slots by create_seq descending (ties: ask index)
+        std::vector<uint32_t> iota(m);
+        for (uint32_t i = 0; i < m; ++i) iota[i] = i;
+        PK(cudaMemcpyAsync(d_ask, vask.data(), 4 * (size_t)m, cudaMemcpyHostToDevice, s));
+        PK(cudaMemcpyAsync(d_leaf, vleaf.data(), 4 * (size_t)m, cudaMemcpyHostToDevice, s));
+        PK(cudaMemcpyAsync(d_flag, vflag.data(), 4 * (size_t)m, cudaMemcpyHostToDevice, s));
+        PK(cudaMemcpyAsync(d_node, vnode.data(), 4 * (size_t)m, cudaMemcpyHostToDevice, s));
+        PK(cudaMemcpyAsync(e->pp_vprio.p, vprio.data(), 4 * (size_t)m, cudaMemcpyHostToDevice, s));
+        PK(cudaMemcpyAsync(e->pp_key[0].p, ckey.data(), 8 * (size_t)m, cudaMemcpyHostToDevice, s));
+        PK(cudaMemcpyAsync(e->pp_tv[0].p, iota.data(), 4 * (size_t)m, cudaMemcpyHostToDevice, s));
+        size_t tb = e->pp_cub.n;
+        PK(cub::DeviceRadixSort::SortPairs(e->pp_cub.p, tb, e->pp_key[0].p, e->pp_key[1].p, e->pp_tv[0].p, d_perm, (int)m, 0, 64, s));
+        PK(cudaMemcpyAsync(perm.data(), d_perm, 4 * (size_t)m, cudaMemcpyDeviceToHost, s));
+        PK(cudaStreamSynchronize(s));
+        e->st.other_launches += 10;
+        e->st.h2d_bytes += 32 * (size_t)m;
+        e->st.d2h_bytes += 4 * (size_t)m;
+    }
+    YkPPArgs pa{};
+    pa.D = D;
+    pa.q_parent = e->pp_q32.p; pa.q_depth = e->pp_q32.p + nq; pa.q_tin = e->pp_q32.p + 2 * (size_t)nq; pa.q_tout = e->pp_q32.p + 3 * (size_t)nq;
+    pa.q_poff = e->pp_q64.p; pa.q_guar = e->pp_q64.p + nq; pa.q_use = e->pp_q64.p + (size_t)nq * (1 + D); pa.q_hasg = e->pp_hasg.p; pa.nq = (int)nq;
+    pa.v_ask = d_ask; pa.v_leaf = d_leaf; pa.v_prio = e->pp_vprio.p; pa.v_flag = d_flag; pa.v_node = d_node; pa.perm = d_perm; pa.m = (int)m;
+    pa.pos = e->pn_pos.p; pa.sorted = e->f_val_out.p; pa.nlive = (int)nlive; pa.room = e->pp_room.p;
+    pa.total = e->d_total.p; pa.ldn = N; pa.taint = e->d_taint.p; pa.label = e->d_label.p; pa.flags = e->d_flags.p;
+    pa.a_req = e->d_areq.p; pa.a_tol = e->d_atol.p; pa.a_need = e->d_aneed.p; pa.a_deny = e->d_adeny.p; pa.lda = e->maxA;
+
+    // ---- host side of the rules ----
+    std::vector<int64_t> rem((size_t)D * nq, 0);   // what the victims taken for the current preemptor remove, per queue
+    std::vector<uint32_t> touched, tstamp(m, 0);
+    uint32_t stamp = 0;
+    uint32_t L = 0;
+    auto rule5 = [&](uint32_t sl) {
+        const uint32_t x = vleaf[sl], v = vask[sl], c = yk_pp_lca(par, depth, x, L);
+        for (uint32_t q = x; q != c; q = par[q]) {
+            if (!hasg[q]) continue;
+            for (int k = 0; k < D; ++k) {
+                const int64_t gq = guar[(size_t)k * nq + q];
+                if (gq >= 0 && use[(size_t)k * nq + q] - rem[(size_t)k * nq + q] - req(v, k) < gq) return false;
+            }
+        }
+        return true;
+    };
+    auto take = [&](uint32_t sl, std::vector<uint32_t>& out) {
+        out.push_back(vask[sl]);
+        tstamp[sl] = stamp;
+        for (uint32_t q = vleaf[sl]; q != YK_NONE; q = par[q]) {
+            touched.push_back(q);
+            for (int k = 0; k < D; ++k) rem[(size_t)k * nq + q] += req(vask[sl], k);
+        }
+    };
+    auto user_over = [&](uint32_t a) {
+        const uint32_t p = e->a_app[a];
+        if (!e->n_ul || e->p_user[p] == YK_NONE) return false;
+        for (uint32_t l = 0; l < e->n_ul; ++l) {
+            if (e->ul_user[l] != e->p_user[p]) continue;
+            bool on_chain = false;
+            for (uint32_t q = leaf_of(a); q != YK_NONE && !on_chain; q = par[q]) on_chain = q == e->ul_queue[l];
+            if (!on_chain) continue;
+            for (int k = 0; k < D; ++k) {
+                const int64_t mx = e->ul_max[(size_t)k * e->n_ul + l];
+                if (mx >= 0 && e->ul_alloc[(size_t)k * e->n_ul + l] + req(a, k) > mx) return true;
+            }
+        }
+        return false;
+    };
+    uint32_t voff = 0, done = 0;
+    std::vector<uint32_t> pnode; std::vector<int64_t> pval;
+    std::vector<uint32_t> seg(2), segv, elig, v6, v7;
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t a = asks[i];
+        const uint8_t st = e->a_state[a];
+        uint32_t status = YK_PP_NO_VICTIMS, node = YK_NONE;
+        v6.clear(); v7.clear();
+        for (uint32_t q : touched) for (int k = 0; k < D; ++k) rem[(size_t)k * nq + q] = 0;
+        touched.clear();
+        if (++stamp == 0) { std::fill(tstamp.begin(), tstamp.end(), 0u); stamp = 1; }
+        // rule 1: who may preempt
+        if (st == yk::ST_ABSENT || (st != yk::ST_NOFIT && st != yk::ST_SKIPPED) || e->pp_plan[a] != YK_NONE) status = YK_PP_NOT_BLOCKED;
+        else if (e->a_flags[a] & YK_ASK_NO_PREEMPT_OTHER) status = YK_PP_NOT_ALLOWED;
+        else if ((e->a_flags[a] & YK_ASK_SLOWPATH) || e->a_gang[a] != YK_NONE || e->a_node[a] != YK_NONE) status = YK_PP_UNSUPPORTED;
+        else if (user_over(a)) status = YK_PP_NOT_ALLOWED;
+        else {
+            // rule 2: the preemptor's own guarantee
+            L = leaf_of(a);
+            bool ok = hasg[L] != 0;
+            for (uint32_t q = L; q != YK_NONE && ok; q = par[q])
+                for (int k = 0; k < D && ok; ++k) {
+                    const int64_t gq = guar[(size_t)k * nq + q];
+                    if (gq >= 0 && use[(size_t)k * nq + q] + req(a, k) > gq) ok = false;
+                }
+            if (!ok) status = YK_PP_GUARANTEE;
+        }
+        if (status == YK_PP_NO_VICTIMS && nlive) {
+            // rules 3-6 on the device
+            uint32_t fence = 0;
+            for (uint32_t q = L; q != YK_NONE; q = par[q]) if (e->q_pp_fence[q]) { fence = q; break; }
+            pa.ask = a; pa.leaf = L; pa.fence = fence; pa.prio = e->a_prio[a];
+            PK(cudaMemcpyAsync(e->pp_q64.p + (size_t)nq * (1 + D), use, 8 * (size_t)D * nq, cudaMemcpyHostToDevice, s));
+            PK(cudaMemsetAsync(e->pp_cnt.p, 0, 4, s));
+            PK(cudaMemsetAsync(e->pp_best.p, 0xFF, 8, s));
+            e->st.h2d_bytes += 8 * (size_t)D * nq;
+            if (m) {
+                const unsigned blocks = (m + 255) / 256;
+                yk_pp_victim_kernel<<<blocks, 256, 0, s>>>(pa, e->pp_key[0].p, e->pp_tv[0].p, e->pp_cnt.p);
+                size_t tb = e->pp_cub.n;
+                PK(cub::DeviceRadixSort::SortPairs(e->pp_cub.p, tb, e->pp_key[0].p, e->pp_key[1].p, e->pp_tv[0].p, e->pp_tv[1].p, (int)m, 0, 64, s));
+                yk_pp_nodekey_kernel<<<blocks, 256, 0, s>>>(pa, e->pp_key[1].p, e->pp_tv[1].p, e->pp_nkey[0].p, e->pp_nval[0].p);
+                tb = e->pp_cub.n;   // stable: a node's entries stay in victim order
+                PK(cub::DeviceRadixSort::SortPairs(e->pp_cub.p, tb, e->pp_nkey[0].p, e->pp_nkey[1].p, e->pp_nval[0].p, e->pp_nval[1].p, (int)m, 0, nbits, s));
+                e->st.other_launches += 2 + 10 + 2 + (nbits + 7) / 8;
+            }
+            yk_pp_node_kernel<<<(nlive + 3) / 4, 128, 0, s>>>(pa, e->pp_nkey[1].p, e->pp_nval[1].p, e->pp_taken.p, e->pp_seg.p, e->pp_best.p);
+            PK(cudaGetLastError());
+            unsigned long long best = 0; uint32_t cnt = 0;
+            PK(cudaMemcpyAsync(&best, e->pp_best.p, 8, cudaMemcpyDeviceToHost, s));
+            PK(cudaMemcpyAsync(&cnt, e->pp_cnt.p, 4, cudaMemcpyDeviceToHost, s));
+            PK(cudaStreamSynchronize(s));
+            e->st.other_launches += 1;
+            e->st.d2h_bytes += 12;
+            if (best != ~0ull) {
+                const uint32_t p = (uint32_t)best, need = (uint32_t)(best >> 32);
+                node = order[p];
+                if (need) {   // the chosen node's victims: its segment again, rule 5 on the host
+                    PK(cudaMemcpyAsync(seg.data(), e->pp_seg.p + 2 * (size_t)p, 8, cudaMemcpyDeviceToHost, s));
+                    PK(cudaStreamSynchronize(s));
+                    segv.resize(seg[1] - seg[0]);
+                    PK(cudaMemcpyAsync(segv.data(), e->pp_nval[1].p + seg[0], 4 * segv.size(), cudaMemcpyDeviceToHost, s));
+                    PK(cudaStreamSynchronize(s));
+                    e->st.d2h_bytes += 8 + 4 * segv.size();
+                    int64_t r[8];
+                    for (int k = 0; k < D; ++k) r[k] = room[(size_t)k * N + node];
+                    for (uint32_t t : segv) {
+                        const uint32_t sl = perm[t];
+                        if (!rule5(sl)) continue;
+                        take(sl, v6);
+                        bool fit = true;
+                        for (int k = 0; k < D; ++k) { r[k] += req(vask[sl], k); fit = fit && req(a, k) <= std::max<int64_t>(0, r[k]); }
+                        if (fit) break;
+                    }
+                    if (v6.size() != need) return bail(e->fail(YK_ERR_STATE, "yk_preemption_plan: device and host victim walks differ"));
+                }
+                // rule 7: queues on the path over their max
+                auto deficit = [&](uint32_t q) {
+                    for (int k = 0; k < D; ++k) {
+                        const int64_t mx = e->q_max[(size_t)k * nq + q];
+                        if (mx >= 0 && use[(size_t)k * nq + q] - rem[(size_t)k * nq + q] + req(a, k) > mx) return true;
+                    }
+                    return false;
+                };
+                std::vector<uint32_t> over;
+                for (uint32_t q = L; q != YK_NONE; q = par[q]) if (deficit(q)) over.push_back(q);
+                if (!over.empty()) {
+                    elig.resize(cnt);
+                    if (cnt) PK(cudaMemcpyAsync(elig.data(), e->pp_tv[1].p, 4 * (size_t)cnt, cudaMemcpyDeviceToHost, s));
+                    PK(cudaStreamSynchronize(s));
+                    e->st.d2h_bytes += 4 * (size_t)cnt;
+                    for (uint32_t t : elig) {
+                        const uint32_t sl = perm[t];
+                        if (tstamp[sl] == stamp) continue;
+                        bool under = false;
+                        for (uint32_t q : over) under = under || yk_pp_inside(tin, tout, q, vleaf[sl]);
+                        if (!under || !rule5(sl)) continue;
+                        take(sl, v7);
+                        over.erase(std::remove_if(over.begin(), over.end(), [&](uint32_t q) { return !deficit(q); }), over.end());
+                        if (over.empty()) break;
+                    }
+                }
+                if (!over.empty()) node = YK_NONE;   // the headroom cannot be freed: no plan
+                else status = v6.empty() && v7.empty() ? YK_PP_FITS : YK_PP_PLANNED;
+            }
+        }
+        const uint32_t nv = (uint32_t)(v6.size() + v7.size());
+        if (status == YK_PP_PLANNED && (uint64_t)voff + nv > victims_cap) break;   // stops before this ask
+        status_out[i] = status;
+        node_out[i] = status == YK_PP_PLANNED || status == YK_PP_FITS ? node : YK_NONE;
+        victim_off_out[i] = voff;
+        if (status == YK_PP_PLANNED) {
+            // rule 8: mark, plan, and bring usage, room and the device copies up to date for the next preemptor
+            pnode.clear(); pval.clear();
+            auto patch = [&](uint32_t x) { pnode.push_back(x); };
+            for (const auto* lst : {&v6, &v7})
+                for (uint32_t v : *lst) {
+                    victims_out[voff++] = v;
+                    e->pp_mark[v] = 1;
+                    chain_add(v, -1);
+                    for (int k = 0; k < D; ++k) room[(size_t)k * N + e->a_bound[v]] += req(v, k);
+                    patch(e->a_bound[v]);
+                    vflag[slot_of[v]] |= YK_PPF_OUT;
+                    PK(cudaMemcpyAsync(d_flag + slot_of[v], &vflag[slot_of[v]], 4, cudaMemcpyHostToDevice, s));
+                }
+            e->pp_plan[a] = node;
+            chain_add(a, +1);
+            for (int k = 0; k < D; ++k) room[(size_t)k * N + node] -= req(a, k);
+            patch(node);
+            std::sort(pnode.begin(), pnode.end());
+            pnode.erase(std::unique(pnode.begin(), pnode.end()), pnode.end());
+            const size_t np = pnode.size();
+            pval.resize((size_t)D * np);
+            for (size_t j = 0; j < np; ++j) for (int k = 0; k < D; ++k) pval[(size_t)k * np + j] = room[(size_t)k * N + pnode[j]];
+            PK(cudaMemcpyAsync(e->pp_pnode.p, pnode.data(), 4 * np, cudaMemcpyHostToDevice, s));
+            PK(cudaMemcpyAsync(e->pp_pval.p, pval.data(), 8 * pval.size(), cudaMemcpyHostToDevice, s));
+            yk_apply_avail_kernel<<<(unsigned)((np + 255) / 256), 256, 0, s>>>(D, e->pp_room.p, N, e->pp_pnode.p, e->pp_pval.p, (int)np);
+            PK(cudaGetLastError());
+            PK(cudaStreamSynchronize(s));   // the staged vectors change with the next preemptor
+            e->st.other_launches += 1;
+            e->st.h2d_bytes += 4 * (size_t)nv + 4 * np + 8 * pval.size();
+        }
+        done = i + 1;
+    }
+#undef PK
+    victim_off_out[done] = voff;
+    *n_done = done;
     return YK_OK;
 }
 

@@ -18,13 +18,20 @@ ST_ABSENT = 255
 YK_ERR_CUDA = -2
 FILTER_SLOTS = 11          # yk_filter_nodes counts: 0 passes, 1..9 YK_FAIL_*, 10 node reserved
 FILTER_RESERVED = 10
+ASK_SLOWPATH = 1
+ASK_NO_PREEMPT_SELF = 2    # not AllowPreemptSelf
+ASK_NO_PREEMPT_OTHER = 4   # not AllowPreemptOther (preemptionPolicy: Never)
+ASK_ORIGINATOR = 8
+# yk_preemption_plan statuses
+PP_PLANNED, PP_FITS, PP_NOT_BLOCKED, PP_NOT_ALLOWED, PP_UNSUPPORTED, PP_GUARANTEE, PP_NO_VICTIMS = range(7)
 
 EXPORTS = [
     "yk_abi_version", "yk_create", "yk_destroy", "yk_nodes_upsert", "yk_nodes_remove", "yk_queues_set", "yk_queues_priority",
-    "yk_apps_upsert", "yk_apps_remove", "yk_apps_user", "yk_user_limits_set", "yk_asks_upsert", "yk_asks_remove", "yk_release",
+    "yk_queues_preemption", "yk_apps_upsert", "yk_apps_remove", "yk_apps_user", "yk_user_limits_set", "yk_asks_upsert",
+    "yk_asks_remove", "yk_release",
     "yk_asks_resize", "yk_cycle",
     "yk_ask_states", "yk_nodes_available", "yk_evaluate", "yk_evaluate_reserve", "yk_node_scores", "yk_node_sort_set", "yk_filter_nodes",
-    "yk_preemption_search", "yk_preemption_nodes", "yk_set_exchange",
+    "yk_preemption_search", "yk_preemption_nodes", "yk_preemption_plan", "yk_set_exchange",
     "yk_peer_export", "yk_peer_import", "yk_peer_enable", "yk_stats",
     "yk_stats_reset", "yk_strerror", "yk_last_error",
 ]
@@ -159,6 +166,7 @@ class Engine:
         if binpacking_device:
             cfg.flags |= FLAG_BINPACKING_DEVICE
         self.D = D
+        self.max_asks = max_asks
         self._h = C.c_void_p()
         rc = self._lib.yk_create(C.byref(cfg), C.byref(self._h))
         if rc != 0:
@@ -205,6 +213,7 @@ class Engine:
         par[par < 0] = YK_NONE
         par = par.astype(np.uint32)
         q = par.size
+        self.n_queues = q
         g = None if guaranteed is None else _colmajor(guaranteed, self.D, q)
         m = None if max is None else _colmajor(max, self.D, q)
         al = None if allocated is None else _colmajor(allocated, self.D, q)
@@ -216,6 +225,12 @@ class Engine:
         fen = _arr(np.asarray(fence).astype(np.uint8), np.uint8) if fence is not None else None
         q = off.size if off is not None else (fen.size if fen is not None else 0)
         self._ck(self._lib.yk_queues_priority(self._h, C.c_uint32(q), _p(off), _p(fen)))
+
+    def queues_preemption(self, fence=None):
+        """queue property preemption.policy == fence ([Q] bool, None = no fence); call after queues_set"""
+        fen = _arr(np.asarray(fence).astype(np.uint8), np.uint8) if fence is not None else None
+        q = fen.size if fen is not None else getattr(self, "n_queues", 0)
+        self._ck(self._lib.yk_queues_preemption(self._h, C.c_uint32(q), _p(fen)))
 
     def apps_upsert(self, idx, queue, submit_time):
         idx = _arr(idx, np.uint32)
@@ -362,6 +377,22 @@ class Engine:
                                                C.c_uint32(skip), C.c_uint32(k), _p(nodes) if k else None, _p(need) if k else None,
                                                _p(n_fit), _p(best_node), _p(best_need)))
         return nodes, need, n_fit, best_node, best_need
+
+    def preemption_plan(self, asks, victims_cap=None):
+        """plan preemption for the preemptors in order -> (status[d], node[d], victims: d arrays of ask indices, d = n_done);
+        victims_cap (default max_asks) bounds the victims of the whole call: planning stops before the ask that would pass it"""
+        asks = _arr(asks, np.uint32)
+        n = asks.size
+        cap = self.max_asks if victims_cap is None else int(victims_cap)
+        status = np.zeros(max(n, 1), dtype=np.uint32)
+        node = np.zeros(max(n, 1), dtype=np.uint32)
+        off = np.zeros(n + 1, dtype=np.uint32)
+        vic = np.zeros(max(cap, 1), dtype=np.uint32)
+        done = C.c_uint32(0)
+        self._ck(self._lib.yk_preemption_plan(self._h, C.c_uint32(n), _p(asks), _p(status), _p(node), _p(off),
+                                              _p(vic) if cap else None, C.c_uint32(cap), C.byref(done)))
+        d = done.value
+        return status[:d].copy(), node[:d].copy(), [vic[off[i]:off[i + 1]].copy() for i in range(d)], d
 
     def set_exchange(self, fn):
         cb = ALLGATHER_FN(fn) if fn is not None else C.cast(None, ALLGATHER_FN)

@@ -125,8 +125,35 @@ class World:
         self.plans.pop(a, None)
 
     def resize(self, a, new):
-        self.req[a] = [int(x) for x in new]
+        """an allocation moves by new - old in its node (while present), queues and user entries; a pending ask's plan goes"""
+        new = [int(x) for x in new]
+        if a in self.bound:
+            n = self.bound[a]
+            d = [new[k] - self.req[a][k] for k in range(self.D)]
+            for k in range(self.D):
+                if n in self.present_nodes:
+                    self.avail[n][k] -= d[k]
+            for q in self.path(self.leaf(a)):
+                for k in range(self.D):
+                    self.alloc[q][k] += d[k]
+            for (_, _, _, held) in self.ul_of(a):
+                for k in range(self.D):
+                    held[k] += d[k]
+        self.req[a] = new
         self.plans.pop(a, None)
+
+    def node_upsert(self, n, total, avail, taint=0, label=0, flags=1):
+        """yk_nodes_upsert of one node: its tables are what is given (a removed node comes back with them)"""
+        s = self.s
+        s.node_total[n] = total
+        s.node_taint[n], s.node_label[n], s.node_flags[n] = taint, label, flags
+        self.avail[n] = [int(x) for x in avail]
+        self.present_nodes.add(n)
+
+    def node_remove(self, n):
+        """yk_nodes_remove: allocations bound there stay allocated, but are no victims and give nothing back on release"""
+        self.present_nodes.discard(n)
+        self.s.node_flags[n] = 0
 
     # ---- plan-call views ----
     def usage(self, q):
@@ -139,6 +166,15 @@ class World:
                 u = [u[k] + self.req[p][k] for k in range(self.D)]
         return u
 
+    def usages(self):
+        """usage(q) of every queue, in one pass"""
+        u = [list(row) for row in self.alloc]
+        for v, sign in [(v, -1) for v in self.marked] + [(p, 1) for p in self.plans]:
+            for q in self.path(self.leaf(v)):
+                for k in range(self.D):
+                    u[q][k] += sign * self.req[v][k]
+        return dict(enumerate(u))
+
     def room(self, n):
         r = list(self.avail[n])
         for v in self.marked:
@@ -147,6 +183,15 @@ class World:
         for p, pn in self.plans.items():
             if pn == n:
                 r = [r[k] - self.req[p][k] for k in range(self.D)]
+        return r
+
+    def rooms(self):
+        """room(n) of every present node, in one pass"""
+        r = {n: list(self.avail[n]) for n in self.present_nodes}
+        for v, n, sign in [(v, self.bound[v], 1) for v in self.marked] + [(p, n, -1) for p, n in self.plans.items()]:
+            if n in r:
+                for k in range(self.D):
+                    r[n][k] += sign * self.req[v][k]
         return r
 
     def node_order(self):
@@ -177,13 +222,17 @@ def _has_guarantee(w, q):
 
 def plan(w, asks, info=None):
     """-> [(status, node or None, [victims])] per ask handled, marking and planning in w as the engine does.  info (a list):
-    one dict per plan made -- victims needed on the node, headroom victims bound elsewhere, whether an earlier ask of the
-    same call was planned -- for the tests' coverage counts"""
+    one dict per plan made, for the tests' coverage counts: victims needed on the node, headroom victims bound elsewhere,
+    whether an earlier ask of the same call was planned, whether a node that fails only the cordon / taint / label steps
+    would have needed fewer victims (or as few, earlier in the order), how many allocations on the node would be victims but for
+    their required node, whether an int32 wrap instead of the clamp would reorder the node's victims, the victim-order
+    position of the last headroom victim, and whether two victims share a create time"""
     out = []
     order = w.node_order() if w.present_nodes else []
+    s = w.s
+    D = w.D
     for a in asks:
         a = int(a)
-        s = w.s
         st = w.state.get(a, 255)
         fl = int(s.ask_flags[a])
         if st not in (ST_NOFIT, ST_SKIPPED) or a in w.plans:
@@ -195,13 +244,13 @@ def plan(w, asks, info=None):
         if (fl & 1) or int(s.ask_gang[a]) >= 0 or int(s.ask_node[a]) >= 0:
             out.append((UNSUPPORTED, None, []))
             continue
-        if any(held[k] + w.req[a][k] > mx[k] for (_, _, mx, held) in w.ul_of(a) for k in range(w.D) if mx[k] >= 0):
+        if any(held[k] + w.req[a][k] > mx[k] for (_, _, mx, held) in w.ul_of(a) for k in range(D) if mx[k] >= 0):
             out.append((NOT_ALLOWED, None, []))
             continue
         L = w.leaf(a)
-        use = {q: w.usage(q) for q in range(w.Q)}
+        use = w.usages()
         if not _has_guarantee(w, L) or any(w.guar[q][k] >= 0 and use[q][k] + w.req[a][k] > w.guar[q][k]
-                                           for q in w.path(L) for k in range(w.D)):
+                                           for q in w.path(L) for k in range(D)):
             out.append((GUARANTEE, None, []))
             continue
         fence = next((q for q in w.path(L) if w.fence[q]), 0)
@@ -209,21 +258,31 @@ def plan(w, asks, info=None):
         def adjusted(x, prio, c):
             return prio + sum(w.off[q] for q in w.below(x, c))
 
-        victims = []
-        for v in sorted(w.bound):
-            if w.state.get(v) != ST_ALLOCATED or v in w.marked or int(s.ask_node[v]) >= 0 or w.bound[v] not in w.present_nodes:
-                continue
+        def candidate(v):
+            """rule 3 apart from the required node: v's adjusted priority, or None"""
+            if w.state.get(v) != ST_ALLOCATED or v in w.marked or w.bound[v] not in w.present_nodes:
+                return None
             x = w.leaf(v)
             if x == L or fence not in w.path(x):
-                continue
+                return None
             c = w.lca(x, L)
             pv, pa = adjusted(x, int(s.ask_prio[v]), c), adjusted(L, int(s.ask_prio[a]), c)
-            if pv > pa:
+            return None if pv > pa else pv
+
+        victims, required = [], []
+        for v in sorted(w.bound):
+            pv = candidate(v)
+            if pv is None:
+                continue
+            if int(s.ask_node[v]) >= 0:
+                required.append((v, pv))
                 continue
             fv = int(s.ask_flags[v])
             victims.append(((1 if fv & NO_SELF else 0, 1 if fv & ORIGINATOR else 0, min(max(pv, I32[0]), I32[1]),
-                             -int(s.ask_create[v]), v), v))
-        victims = [v for _, v in sorted(victims)]
+                             -int(s.ask_create[v]), v), v, pv))
+        victims.sort()
+        adj = {v: pv for _, v, pv in victims}
+        victims = [v for _, v, _ in victims]
 
         def allowed(v, taken):
             """rule 5: v may go once `taken` are gone"""
@@ -231,32 +290,55 @@ def plan(w, asks, info=None):
             for q in w.below(x, w.lca(x, L)):
                 if not _has_guarantee(w, q):
                     continue
-                gone = [sum(w.req[t][k] for t in taken + [v] if q in w.path(w.leaf(t))) for k in range(w.D)]
-                if any(w.guar[q][k] >= 0 and use[q][k] - gone[k] < w.guar[q][k] for k in range(w.D)):
+                gone = [sum(w.req[t][k] for t in taken + [v] if q in w.path(w.leaf(t))) for k in range(D)]
+                if any(w.guar[q][k] >= 0 and use[q][k] - gone[k] < w.guar[q][k] for k in range(D)):
                     return False
             return True
 
         def fits(r):
-            return all(w.req[a][k] <= max(0, r[k]) for k in range(w.D))
+            return all(w.req[a][k] <= max(0, r[k]) for k in range(D))
 
-        best = None
-        for n in order:
-            if not w.static_ok(a, n):
-                continue
-            r = w.room(n)
+        rooms = w.rooms()
+        on_node = {}
+        for v in victims:
+            on_node.setdefault(w.bound[v], []).append(v)
+
+        def walk(n):
+            """rule 6 on node n: the fewest victims in order after which the ask fits, or None"""
+            r = list(rooms[n])
             taken = []
             if not fits(r):
-                for v in victims:
-                    if w.bound[v] != n or not allowed(v, taken):
+                for v in on_node.get(n, []):
+                    if not allowed(v, taken):
                         continue
                     taken.append(v)
-                    r = [r[k] + w.req[v][k] for k in range(w.D)]
+                    r = [r[k] + w.req[v][k] for k in range(D)]
                     if fits(r):
                         break
                 if not fits(r):
-                    continue
-            if best is None or len(taken) < len(best[1]):
+                    return None
+            return taken
+
+        def masks_ok(n):
+            return w.static_ok(a, n)
+
+        def total_ok(n):
+            return all(w.req[a][k] <= max(0, int(s.node_total[n][k])) for k in range(D))
+
+        best, masked = None, None
+        for n in order:
+            if not total_ok(n):
+                continue
+            ok = masks_ok(n)
+            if not ok and info is None:
+                continue
+            taken = walk(n)
+            if taken is None:
+                continue
+            if ok and (best is None or len(taken) < len(best[1])):
                 best = (n, taken)
+            if masked is None or len(taken) < len(masked[1]):
+                masked = (n, taken, ok)
         if best is None:
             out.append((NO_VICTIMS, None, []))
             continue
@@ -264,8 +346,8 @@ def plan(w, asks, info=None):
         taken = list(v6)
 
         def over(q):
-            gone = [sum(w.req[t][k] for t in taken if q in w.path(w.leaf(t))) for k in range(w.D)]
-            return any(w.qmax[q][k] >= 0 and use[q][k] - gone[k] + w.req[a][k] > w.qmax[q][k] for k in range(w.D))
+            gone = [sum(w.req[t][k] for t in taken if q in w.path(w.leaf(t))) for k in range(D)]
+            return any(w.qmax[q][k] >= 0 and use[q][k] - gone[k] + w.req[a][k] > w.qmax[q][k] for k in range(D))
 
         v7 = []
         for v in victims:
@@ -283,8 +365,21 @@ def plan(w, asks, info=None):
             out.append((FITS, node, []))
             continue
         if info is not None:
-            info.append(dict(need=len(v6), off_node=sum(1 for v in v7 if w.bound[v] != node),
-                             after_plan=any(x[0] == PLANNED for x in out)))
+            mine = on_node.get(node, [])
+            last = mine.index(v6[-1]) if v6 else -1
+            walked_key = {v: (min(max(adj[v], I32[0]), I32[1]), -int(s.ask_create[v]), v) for v in mine}
+            wrapped_key = {v: ((adj[v] + (1 << 31)) % (1 << 32) - (1 << 31), -int(s.ask_create[v]), v) for v in mine}
+            flags = {v: (int(s.ask_flags[v]) & NO_SELF, int(s.ask_flags[v]) & ORIGINATOR) for v in mine}
+            creates = [int(s.ask_create[v]) for v in taken]
+            info.append(dict(
+                need=len(v6), off_node=sum(1 for v in v7 if w.bound[v] != node),
+                after_plan=any(x[0] == PLANNED for x in out),
+                masked=masked[2] is False,
+                required_skipped=sum(1 for v, _ in required if w.bound[v] == node) if v6 else 0,
+                clamp_decides=bool(v6) and sorted(mine, key=lambda v: (flags[v], walked_key[v]))[:last + 1]
+                != sorted(mine, key=lambda v: (flags[v], wrapped_key[v]))[:last + 1],
+                pos7=max((victims.index(v) for v in v7), default=-1),
+                create_ties=len(set(creates)) < len(creates)))
         out.append((PLANNED, node, taken))
         w.marked.update(taken)
         w.plans[a] = node

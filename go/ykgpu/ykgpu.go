@@ -88,6 +88,8 @@ type askRec struct {
 	ppFlags   C.uint32_t // YK_ASK_NO_PREEMPT_SELF / _OTHER / YK_ASK_ORIGINATOR from the ask's PreemptionPolicy and Originator
 	blocked   time.Time  // when the ask was first reported NOFIT / SKIPPED since it last was anything else (zero: not blocked)
 	pinNode   uint32     // none, or the node a preemption plan holds for it: written as its required node
+	dsNode    string     // a DaemonSet pod's node (CreateTagsForTask's required node), "" otherwise; apart from pinNode
+	dsPlanned bool       // yk_preemption_required_node planned it; cleared when it is written again
 }
 
 type Engine struct {
@@ -686,13 +688,38 @@ func needsGoPredicates(p *v1.Pod) bool {
 	return len(p.Spec.TopologySpreadConstraints) > 0
 }
 
+// daemonSetNode: the required node of a DaemonSet pod as the shim's CreateTagsForTask finds it (pkg/common/si_helper.go:33-58):
+// for an owner of kind DaemonSet, the last metadata.name match field of its required node affinity, first value; "" when
+// there is none
+func daemonSetNode(p *v1.Pod) string {
+	node := ""
+	for _, o := range p.GetOwnerReferences() {
+		if o.Kind != "DaemonSet" {
+			continue
+		}
+		a := p.Spec.Affinity
+		if a == nil || a.NodeAffinity == nil || a.NodeAffinity.RequiredDuringSchedulingIgnoredDuringExecution == nil {
+			continue
+		}
+		for _, t := range a.NodeAffinity.RequiredDuringSchedulingIgnoredDuringExecution.NodeSelectorTerms {
+			for _, m := range t.MatchFields {
+				if m.Key == "metadata.name" && len(m.Values) > 0 {
+					node = m.Values[0]
+				}
+			}
+		}
+	}
+	return node
+}
+
 // podMasks: nodeSelector + required node affinity + tolerations + spec.nodeName -> yk_pod_masks.  exact: the dictionary
-// encoded all of them (it did not set YK_ASK_SLOWPATH itself; needsGoPredicates may still have)
-func (e *Engine) podMasks(p *v1.Pod) (out C.yk_pod_masks, exact bool) {
+// encoded all of them (it did not set YK_ASK_SLOWPATH itself; needsGoPredicates may still have).  A DaemonSet pod is encoded
+// against its node (yk_dict_pod_required_node), which also becomes its required node; dsNode names it.
+func (e *Engine) podMasks(p *v1.Pod) (out C.yk_pod_masks, exact bool, dsNode string) {
 	out.required_node = C.YK_NONE
 	if p == nil {
 		out.flags = C.YK_ASK_SLOWPATH
-		return out, false
+		return out, false, ""
 	}
 	var held []unsafe.Pointer
 	hold := func(s string) *C.char { c := C.CString(s); held = append(held, unsafe.Pointer(c)); return c }
@@ -766,12 +793,16 @@ func (e *Engine) podMasks(p *v1.Pod) (out C.yk_pod_masks, exact bool) {
 	if p.Spec.NodeName != "" {
 		spec.node_name = hold(p.Spec.NodeName)
 	}
-	C.yk_dict_pod(e.dict, &spec, &out)
+	if dsNode = daemonSetNode(p); dsNode != "" {
+		C.yk_dict_pod_required_node(e.dict, &spec, hold(dsNode), &out)
+	} else {
+		C.yk_dict_pod(e.dict, &spec, &out)
+	}
 	exact = out.flags&C.YK_ASK_SLOWPATH == 0
 	if needsGoPredicates(p) {
 		out.flags |= C.YK_ASK_SLOWPATH
 	}
-	return out, exact
+	return out, exact, dsNode
 }
 
 // dictionary handed out new bits while compiling a pod: node bit sets (and key-only tolerations) were extended
@@ -823,9 +854,10 @@ func (e *Engine) pushAsk(idx uint32, a *askRec, alloc *si.Allocation) error {
 	if e.src != nil {
 		pod = e.src.GetPod(a.key)
 	}
-	m, exact := e.podMasks(pod)
+	m, exact, dsNode := e.podMasks(pod)
 	a.slow = m.flags&C.YK_ASK_SLOWPATH != 0
 	a.exact = exact
+	a.dsNode, a.dsPlanned = dsNode, false // a write clears the engine's plan
 	app, ok := e.appIdx[a.app]
 	if !ok {
 		return fmt.Errorf("ask %s: unknown application %s", a.key, a.app)
@@ -909,6 +941,7 @@ func (e *Engine) resize(idx uint32, req [4]int64) error {
 		return err
 	}
 	a.req = req
+	a.dsPlanned = false // a resize clears the engine's plan
 	return nil
 }
 
@@ -1022,6 +1055,13 @@ func (e *Engine) loop() {
 		if rc == C.YK_OK {
 			states = e.collectStates()
 			preempted = e.preempt()
+			if ds := e.preemptDaemons(); ds != nil {
+				if preempted == nil {
+					preempted = ds
+				} else {
+					preempted.Released = append(preempted.Released, ds.Released...)
+				}
+			}
 		}
 		slowKeys := make([]uint32, 0, int(nslow))
 		for i := 0; i < int(nslow); i++ {
@@ -1058,7 +1098,7 @@ func (e *Engine) preempt() *si.AllocationResponse {
 	var asks []C.uint32_t
 	for i := range e.asks {
 		a := &e.asks[i]
-		if !a.present || a.foreign || a.slow || a.blocked.IsZero() || a.pinNode != none {
+		if !a.present || a.foreign || a.slow || a.blocked.IsZero() || a.pinNode != none || a.dsNode != "" {
 			continue
 		}
 		d := 30 * time.Second
@@ -1101,6 +1141,58 @@ func (e *Engine) preempt() *si.AllocationResponse {
 		p := &e.asks[asks[j]]
 		p.pinNode = uint32(node[j])
 		_ = e.pushAsk(uint32(asks[j]), p, nil)
+	}
+	if len(resp.Released) == 0 {
+		return nil
+	}
+	return resp
+}
+
+// preemptDaemons: the core's required-node preemption (yk_preemption_required_node, DESIGN.md §2 item 10), once per loop, for
+// every DaemonSet ask that ended the cycle NOFIT / SKIPPED and has no plan, oldest blocked first.  There is no
+// preemption.delay: the core's required-node path does not wait.  Only asks with dsNode go there -- never a guarantee-planned
+// preemptor pinned through its required node.  The victims are released here and handed to the shim as preempted; the next
+// cycle places the preemptor on its node.  Called with e.mu held; nil when nothing was preempted.
+func (e *Engine) preemptDaemons() *si.AllocationResponse {
+	var asks []C.uint32_t
+	for i := range e.asks {
+		a := &e.asks[i]
+		if a.present && !a.foreign && !a.slow && a.dsNode != "" && !a.dsPlanned && !a.blocked.IsZero() {
+			asks = append(asks, C.uint32_t(i))
+		}
+	}
+	if len(asks) == 0 {
+		return nil
+	}
+	sort.SliceStable(asks, func(x, y int) bool { return e.asks[asks[x]].blocked.Before(e.asks[asks[y]].blocked) })
+	n := len(asks)
+	status, off := make([]C.uint32_t, n), make([]C.uint32_t, n+1)
+	victims := make([]C.uint32_t, len(e.asks)+1)
+	var done C.uint32_t
+	if e.ck(C.yk_preemption_required_node(e.h, C.uint32_t(n), &asks[0], &status[0], &off[0], &victims[0],
+		C.uint32_t(len(victims)), &done), "yk_preemption_required_node") != nil {
+		return nil
+	}
+	resp := &si.AllocationResponse{}
+	for j := 0; j < int(done); j++ {
+		if status[j] != C.YK_PP_PLANNED {
+			continue
+		}
+		p := &e.asks[asks[j]]
+		p.dsPlanned = true
+		vs := victims[off[j]:off[j+1]]
+		if C.yk_release(e.h, C.uint32_t(len(vs)), &vs[0]) != C.YK_OK {
+			continue
+		}
+		for _, v := range vs {
+			a := &e.asks[v]
+			resp.Released = append(resp.Released, &si.AllocationRelease{ApplicationID: a.app, AllocationKey: a.key,
+				TerminationType: si.TerminationType_PREEMPTED_BY_SCHEDULER,
+				Message:         "preempting allocations to free up resources to run daemon set ask: " + p.key})
+			a.present = false
+			delete(e.askIdx, a.key)
+			e.freeAsks = append(e.freeAsks, uint32(v))
+		}
 	}
 	if len(resp.Released) == 0 {
 		return nil

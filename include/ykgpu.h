@@ -40,6 +40,8 @@
  *   yk_preemption_nodes                 the same search on every node for a list of asks, from the allocations the
  *                                       engine made: the search half of a preemptor (its policy stays with the caller)
  *   yk_preemption_plan                  the core's preemption for queues below their guarantee: victims, node and marks
+ *   yk_preemption_required_node         the core's preemption for asks with a required node (DaemonSet pods): victims on
+ *                                       that node and marks, for a whole rollout in one device pass
  *
  * Conventions: every call returns YK_OK (0) or a negative yk_status; no exceptions or aborts cross the
  * boundary.  Inputs are caller-owned host memory, fully consumed before return (cgo: no Go pointer is
@@ -427,6 +429,37 @@ int yk_preemption_nodes(yk_engine* e, uint32_t n, const uint32_t* asks,
 int yk_preemption_plan(yk_engine* e, uint32_t n, const uint32_t* asks, uint32_t* status_out, uint32_t* node_out,
                        uint32_t* victim_off_out /* [n+1] */, uint32_t* victims_out /* [victims_cap] */, uint32_t victims_cap,
                        uint32_t* n_done);
+
+/* Preemption for asks with a required node (DaemonSet pods): for each preemptor a, in the order given, the victims on its node
+ * X = required_node(a) that let it run (the core's required-node preemption, DESIGN.md §2 item 10), evaluated for every
+ * preemptor of the call in one pass on the device (csrc/yk_preempt_required.cuh).  Marks and plans are those of
+ * yk_preemption_plan, and each call sees the other's; room(X) is as documented there.
+ *   Status per ask (status_out[i], the YK_PP_* values; YK_PP_GUARANTEE is never returned):
+ *     YK_PP_NOT_BLOCKED  not present, state not YK_ST_NOFIT / YK_ST_SKIPPED, or already planned by either plan call;
+ *     YK_PP_UNSUPPORTED  no required node, slow path or gang member;
+ *     YK_PP_NOT_ALLOWED  over the headroom of a queue max on its path or of a user / group limit that applies to it, from what
+ *                        is allocated (marks and plans play no part); YK_ASK_NO_PREEMPT_OTHER is not read;
+ *     YK_PP_NO_VICTIMS   X not present, X fails its static steps (schedulable, taints, labels, request <= max(0, total)), or
+ *                        the eligible victims never add up to the request;
+ *     YK_PP_FITS         request <= max(0, room(X)) in every resource: nothing is marked;
+ *     YK_PP_PLANNED      victims marked, the ask planned on X, room(X) moved by + victims - request for later preemptors.
+ *   Victims: allocations bound to X, not marked, without a required node, with priority <= the preemptor's (no queue offsets),
+ *     and a non-zero request on some resource the preemptor asks for.  Order: neither YK_ASK_NO_PREEMPT_SELF nor
+ *     YK_ASK_ORIGINATOR first, then YK_ASK_NO_PREEMPT_SELF non-originators, then originators; priority ascending; create_seq
+ *     descending; index.  The victims are the shortest prefix of that order whose sum covers the preemptor's full request in
+ *     every resource (not the part room(X) lacks).
+ *   Output: the victims of ask i are victims_out[victim_off_out[i] .. victim_off_out[i+1]), in victim order.  Planning stops
+ *     before the first ask, in the order given, whose victims would pass victims_cap; *n_done = the asks handled, and only
+ *     status_out [0, n_done) and victim_off_out [0, n_done] are written.  Nothing past the stop is marked or planned.
+ *   No node order is used: node scores are not computed and a NaN score elsewhere is no error.
+ *   Errors, all checked before anything is marked; nothing changes on an error:
+ *     YK_ERR_ARG   asks / status_out / victim_off_out / n_done NULL with n > 0, victims_out NULL with victims_cap > 0, an index
+ *                  >= max_asks, the same ask twice.
+ *   A YK_ERR_CUDA rolls every mark and plan of the call back.  n == 0 is YK_OK.  Counted in other_launches / h2d_bytes /
+ *   d2h_bytes.  Multi-GPU split sweep (world > 1): every rank makes the same call between the same two cycles. */
+int yk_preemption_required_node(yk_engine* e, uint32_t n, const uint32_t* asks, uint32_t* status_out,
+                                uint32_t* victim_off_out /* [n+1] */, uint32_t* victims_out /* [victims_cap] */,
+                                uint32_t victims_cap, uint32_t* n_done);
 
 /* multi-GPU exchange hook: called once per batch on every rank, after the local shard's rows of `buf`
  * (device pointer, row-major, `row_bytes` per ask, rows [first_row, first_row+n_rows) are this rank's)

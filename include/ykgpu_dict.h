@@ -77,6 +77,14 @@ int yk_dict_node_remove(yk_dict* d, uint32_t node_idx);
 /* compile a pod; may allocate new bits, which changes node bit sets: compare yk_dict_generation before/after
  * and re-read the nodes with yk_dict_node_bits when it moved */
 int yk_dict_pod(yk_dict* d, const yk_pod_spec* pod, yk_pod_masks* out);
+/* a pod whose node is fixed before it is scheduled (a DaemonSet pod: the node its required affinity names through matchFields
+ * metadata.name): encoded as yk_dict_pod does, with required_node = the index of node_name.  An unknown node_name, or a
+ * pod->node_name that differs from it, sets the impossible bit.  The required-affinity terms are resolved against node_name
+ * first: a term whose matchFields reject it is dropped, a term whose fields accept it keeps only its expressions, and a term
+ * left without expressions matches unconditionally, so the affinity adds no bit (an originally empty term still matches
+ * nothing).  The rest is encoded as yk_dict_pod encodes a term list.  Exact for the only node the ask can use; the usual
+ * DaemonSet pod takes no label bit. */
+int yk_dict_pod_required_node(yk_dict* d, const yk_pod_spec* pod, const char* node_name, yk_pod_masks* out);
 uint64_t yk_dict_generation(const yk_dict* d);
 int yk_dict_node_bits(const yk_dict* d, uint32_t node_idx, uint64_t* label_bits, uint64_t* taint_bits);
 

@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libykgpu.so")
 SOURCES = ["yk_engine.cu", "yk_dict.cpp", "yk_podres.cpp"]
-DEPS = ["yk_engine.cu", "yk_dict.cpp", "yk_podres.cpp", "../../include/ykgpu_pod.h", "yk_kernels.cuh", "yk_filter.cuh", "yk_preempt_nodes.cuh", "yk_preempt_plan.cuh", "yk_lattice.cuh", "yk_lattice.h", "yk_uniform.cuh", "yk_uniform.h", "yk_rounds.cuh", "yk_rounds.h", "yk_spec.cuh", "yk_spec.h", "yk_lattice_host.hpp", "yk_orderer.hpp", "yk_dirty.hpp", "yk_commit.hpp", "yk_score.h", "../../include/ykgpu.h",
+DEPS = ["yk_engine.cu", "yk_dict.cpp", "yk_podres.cpp", "../../include/ykgpu_pod.h", "yk_kernels.cuh", "yk_filter.cuh", "yk_preempt_nodes.cuh", "yk_preempt_plan.cuh", "yk_preempt_required.cuh", "yk_lattice.cuh", "yk_lattice.h", "yk_uniform.cuh", "yk_uniform.h", "yk_rounds.cuh", "yk_rounds.h", "yk_spec.cuh", "yk_spec.h", "yk_lattice_host.hpp", "yk_orderer.hpp", "yk_dirty.hpp", "yk_commit.hpp", "yk_score.h", "../../include/ykgpu.h",
         "../../include/ykgpu_dict.h"]
 
 NVCC_FLAGS = [

@@ -271,8 +271,12 @@ int yk_dict_node_bits(const yk_dict* d, uint32_t idx, uint64_t* label_bits, uint
     return YK_OK;
 }
 
-int yk_dict_pod(yk_dict* d, const yk_pod_spec* pod, yk_pod_masks* out) {
-    if (!d || !pod || !out) return YK_ERR_ARG;
+}  // extern "C"
+
+// yk_dict_pod (at == NULL) and yk_dict_pod_required_node (at = the required node's name): the required-affinity terms are
+// resolved against `at` first -- a term whose matchFields reject it is dropped, one whose fields accept it keeps only its
+// expressions, and one left with no expression matches unconditionally
+static int encode_pod(yk_dict* d, const yk_pod_spec* pod, const char* at, yk_pod_masks* out) {
     uint64_t need = 0, deny = 0, tol = 0;
     uint32_t flags = 0, want_node = YK_NONE;
     auto need_bit = [&](int b) { if (b < 0) flags |= YK_ASK_SLOWPATH; else need |= 1ull << b; };
@@ -293,12 +297,28 @@ int yk_dict_pod(yk_dict* d, const yk_pod_spec* pod, yk_pod_masks* out) {
     // required node affinity
     if (pod->has_required_affinity) {
         std::vector<Term> terms;
+        bool always = false;
         for (uint32_t i = 0; i < pod->n_terms; ++i) {
             const yk_selector_term& t = pod->terms[i];
             if (t.n_expressions == 0 && t.n_fields == 0) continue;   // nil or empty term selects no objects
-            terms.push_back(parse_term(t));
+            Term pt = parse_term(t);
+            if (at && !pt.fields.empty()) {
+                bool accept = true;
+                for (const Req& q : pt.fields) {
+                    if (!q.valid) { accept = false; break; }
+                    const bool eq = (q.key == "metadata.name" ? std::string(at) : std::string()) == q.values[0];
+                    if (q.op == YK_OP_IN ? !eq : eq) accept = false;
+                }
+                if (!accept) continue;
+                pt.fields.clear();
+                pt.parse_error = false;
+                for (const Req& q : pt.exprs) if (!q.valid) pt.parse_error = true;
+                if (pt.exprs.empty()) always = true;
+            }
+            terms.push_back(std::move(pt));
         }
-        if (terms.empty()) need |= IMPOSSIBLE;   // nil / empty term list matches nothing
+        if (always) {}                            // a term matches the node whatever its labels: no bit
+        else if (terms.empty()) need |= IMPOSSIBLE;   // nil / empty term list matches nothing
         else if (terms.size() == 1 && terms[0].fields.empty()) {
             if (terms[0].parse_error) need |= IMPOSSIBLE;
             else for (const Req& q : terms[0].exprs) {
@@ -325,14 +345,30 @@ int yk_dict_pod(yk_dict* d, const yk_pod_spec* pod, yk_pod_masks* out) {
     else for (size_t b = 0; b < d->taints.size(); ++b)
         for (uint32_t i = 0; i < pod->n_tolerations; ++i)
             if (tolerates(pod->tolerations[i], d->taints[b])) { tol |= 1ull << b; break; }
-    // pod.Spec.NodeName
-    if (pod->node_name && pod->node_name[0]) {
+    // pod.Spec.NodeName, and the required node
+    if (at) {
+        auto it = d->by_name.find(at);
+        if (it == d->by_name.end()) need |= IMPOSSIBLE; else want_node = it->second;
+        if (pod->node_name && pod->node_name[0] && std::strcmp(pod->node_name, at) != 0) need |= IMPOSSIBLE;
+    } else if (pod->node_name && pod->node_name[0]) {
         auto it = d->by_name.find(pod->node_name);
         if (it == d->by_name.end()) need |= IMPOSSIBLE; else want_node = it->second;
     }
     out->tolerated_bits = tol; out->required_bits = need; out->forbidden_bits = deny;
     out->required_node = want_node; out->flags = flags;
     return YK_OK;
+}
+
+extern "C" {
+
+int yk_dict_pod(yk_dict* d, const yk_pod_spec* pod, yk_pod_masks* out) {
+    if (!d || !pod || !out) return YK_ERR_ARG;
+    return encode_pod(d, pod, nullptr, out);
+}
+
+int yk_dict_pod_required_node(yk_dict* d, const yk_pod_spec* pod, const char* node_name, yk_pod_masks* out) {
+    if (!d || !pod || !node_name || !out) return YK_ERR_ARG;
+    return encode_pod(d, pod, node_name, out);
 }
 
 }  // extern "C"

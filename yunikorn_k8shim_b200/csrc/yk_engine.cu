@@ -32,6 +32,7 @@
 #include "yk_filter.cuh"
 #include "yk_preempt_nodes.cuh"
 #include "yk_preempt_plan.cuh"
+#include "yk_preempt_required.cuh"
 #include "yk_lattice.cuh"
 #include "yk_uniform.cuh"
 #include "yk_rounds.cuh"
@@ -329,6 +330,9 @@ struct yk_engine {
     Dev<uint32_t> pp_q32, pp_v32, pp_tv[2], pp_nkey[2], pp_nval[2], pp_seg, pp_cnt, pp_pnode; Dev<int32_t> pp_vprio;
     Dev<int64_t> pp_q64, pp_room, pp_pval; Dev<uint64_t> pp_key[2]; Dev<unsigned long long> pp_best;
     Dev<uint8_t> pp_hasg, pp_taken, pp_cub;
+    // yk_preemption_required_node: per-call device tables (slots, groups, preemptors, sort buffers, results), grown on demand
+    Dev<uint32_t> prn_u32, prn_val[2], prn_out; Dev<int32_t> prn_i32; Dev<int64_t> prn_room; Dev<uint64_t> prn_key[2];
+    Dev<uint8_t> prn_taken, prn_cub;
     yk_allgather_fn xfn = nullptr; void* xctx = nullptr;
     // peer-to-peer exchange (see yk_peer_export): peers' slot buffers and sync blocks, mapped through CUDA IPC
     bool p2p = false;
@@ -2882,6 +2886,179 @@ int yk_preemption_plan(yk_engine* e, uint32_t n, const uint32_t* asks, uint32_t*
         done = i + 1;
     }
 #undef PK
+    victim_off_out[done] = voff;
+    *n_done = done;
+    return YK_OK;
+}
+
+// The host decides who may preempt (DESIGN.md §2 item 10) and groups the rest by their required node; the device decides every
+// group in one pass (csrc/yk_preempt_required.cuh); the host then applies, in the caller's order, the prefix that fits victims_cap.
+int yk_preemption_required_node(yk_engine* e, uint32_t n, const uint32_t* asks, uint32_t* status_out, uint32_t* victim_off_out,
+                                uint32_t* victims_out, uint32_t victims_cap, uint32_t* n_done) {
+    if (!e) return YK_ERR_ARG;
+    std::lock_guard<std::mutex> g(e->mu);
+    if (n && (!asks || !status_out || !victim_off_out || !n_done))
+        return e->fail(YK_ERR_ARG, "yk_preemption_required_node: null asks, status_out, victim_off_out or n_done");
+    if (victims_cap && !victims_out) return e->fail(YK_ERR_ARG, "yk_preemption_required_node: null victims_out with victims_cap > 0");
+    if (!n) { if (n_done) *n_done = 0; if (victim_off_out) victim_off_out[0] = 0; return YK_OK; }
+    if (e->pn_seen.size() < e->maxA) { e->pn_seen.assign(e->maxA, 0); e->pn_stamp = 0; }
+    if (++e->pn_stamp == 0) { std::fill(e->pn_seen.begin(), e->pn_seen.end(), 0u); e->pn_stamp = 1; }
+    for (uint32_t i = 0; i < n; ++i) {
+        if (asks[i] >= e->maxA) return e->fail(YK_ERR_ARG, "yk_preemption_required_node: ask index beyond max_asks");
+        if (e->pn_seen[asks[i]] == e->pn_stamp) return e->fail(YK_ERR_ARG, "yk_preemption_required_node: the same ask twice");
+        e->pn_seen[asks[i]] = e->pn_stamp;
+    }
+    int rc = upload_tables(e);
+    if (rc) return rc;
+    const int D = e->D;
+    const uint32_t nq = e->nq, A = e->a_hi, N = e->maxN;
+    cudaStream_t s = e->stream;
+    // a plan whose preemptor a cycle has since allocated is spent
+    for (uint32_t a = 0; a < A; ++a) if (e->pp_plan[a] != YK_NONE && e->a_state[a] == yk::ST_ALLOCATED) e->pp_plan[a] = YK_NONE;
+    auto req = [&](uint32_t a, int k) { return e->a_req[(size_t)k * e->maxA + a]; };
+    // over the headroom of a queue max on its path or of a user / group limit that applies to it, from what is allocated
+    auto over = [&](uint32_t a) {
+        const uint32_t p = e->a_app[a];
+        for (uint32_t q = e->p_queue[p]; q != YK_NONE; q = e->q_parent[q])
+            for (int k = 0; k < D; ++k) {
+                const int64_t mx = e->q_max[(size_t)k * nq + q];
+                if (mx >= 0 && e->q_alloc[(size_t)k * nq + q] + req(a, k) > mx) return true;
+            }
+        if (!e->n_ul || e->p_user[p] == YK_NONE) return false;
+        for (uint32_t l = 0; l < e->n_ul; ++l) {
+            if (e->ul_user[l] != e->p_user[p]) continue;
+            bool on_chain = false;
+            for (uint32_t q = e->p_queue[p]; q != YK_NONE && !on_chain; q = e->q_parent[q]) on_chain = q == e->ul_queue[l];
+            if (!on_chain) continue;
+            for (int k = 0; k < D; ++k) {
+                const int64_t mx = e->ul_max[(size_t)k * e->n_ul + l];
+                if (mx >= 0 && e->ul_alloc[(size_t)k * e->n_ul + l] + req(a, k) > mx) return true;
+            }
+        }
+        return false;
+    };
+    // ---- host statuses; the rest grouped by node (groups in order of first appearance, call order inside a group) ----
+    std::vector<uint32_t> status(n, YK_PP_NO_VICTIMS), grp(N, YK_NONE), gnode, gcnt, pgrp(n, YK_NONE);
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t a = asks[i], x = e->a_node[a];
+        const uint8_t st = e->a_state[a];
+        if ((st != yk::ST_NOFIT && st != yk::ST_SKIPPED) || e->pp_plan[a] != YK_NONE) status[i] = YK_PP_NOT_BLOCKED;
+        else if (x == YK_NONE || (e->a_flags[a] & YK_ASK_SLOWPATH) || e->a_gang[a] != YK_NONE) status[i] = YK_PP_UNSUPPORTED;
+        else if (over(a)) status[i] = YK_PP_NOT_ALLOWED;
+        else if (x < N && e->n_present[x]) {
+            if (grp[x] == YK_NONE) { grp[x] = (uint32_t)gnode.size(); gnode.push_back(x); gcnt.push_back(0); }
+            pgrp[i] = grp[x];
+            ++gcnt[grp[x]];
+        }
+    }
+    const uint32_t G = (uint32_t)gnode.size();
+    std::vector<uint32_t> gpoff(G + 1, 0), pask, ppos(n, YK_NONE);
+    std::vector<int32_t> pprio;
+    for (uint32_t gi = 0; gi < G; ++gi) gpoff[gi + 1] = gpoff[gi] + gcnt[gi];
+    const uint32_t P = gpoff[G];
+    pask.resize(P); pprio.resize(P);
+    {
+        std::vector<uint32_t> fill(gpoff.begin(), gpoff.end() - 1);
+        for (uint32_t i = 0; i < n; ++i)
+            if (pgrp[i] != YK_NONE) { const uint32_t at = fill[pgrp[i]]++; ppos[i] = at; pask[at] = asks[i]; pprio[at] = e->a_prio[asks[i]]; }
+    }
+    // room(node) for plan calls, and the slots: allocations on a group's node that may ever be victims, in ask-index order
+    std::vector<int64_t> room((size_t)D * G);
+    for (uint32_t gi = 0; gi < G; ++gi) for (int k = 0; k < D; ++k) room[(size_t)k * G + gi] = e->n_avail[(size_t)k * N + gnode[gi]];
+    std::vector<uint32_t> sask, stg, gseg(G + 1, 0);
+    std::vector<int32_t> sprio;
+    std::vector<uint64_t> ckey;
+    for (uint32_t a = 0; a < A; ++a) {
+        if (e->pp_plan[a] != YK_NONE && e->a_state[a] != yk::ST_ABSENT && grp[e->pp_plan[a]] != YK_NONE)
+            for (int k = 0; k < D; ++k) room[(size_t)k * G + grp[e->pp_plan[a]]] -= req(a, k);
+        const uint32_t x = e->a_bound[a];
+        if (e->a_state[a] != yk::ST_ALLOCATED || x >= N || grp[x] == YK_NONE) continue;
+        if (e->pp_mark[a]) { for (int k = 0; k < D; ++k) room[(size_t)k * G + grp[x]] += req(a, k); continue; }
+        if (e->a_node[a] != YK_NONE) continue;
+        const uint32_t f = e->a_flags[a];
+        const uint32_t type = (f & YK_ASK_ORIGINATOR) ? YK_PRN_TYPE_ORIGINATOR : (f & YK_ASK_NO_PREEMPT_SELF) ? YK_PRN_TYPE_NO_SELF
+                                                                                                               : YK_PRN_TYPE_REGULAR;
+        sask.push_back(a); sprio.push_back(e->a_prio[a]); stg.push_back(type << 30 | grp[x]);
+        ckey.push_back(~((uint64_t)e->a_create[a] ^ (1ull << 63)));   // ascending key = create_seq descending
+        ++gseg[grp[x] + 1];
+    }
+    for (uint32_t gi = 0; gi < G; ++gi) gseg[gi + 1] += gseg[gi];
+    const uint32_t m = (uint32_t)sask.size();
+    if (m >= (1u << 30) || G >= (1u << 30)) return e->fail(YK_ERR_RANGE, "yk_preemption_required_node: 2^30 or more allocations or nodes");
+
+    // ---- one pass on the device for every group ----
+    std::vector<uint32_t> dst(3 * (size_t)P), vout(m);   // status, count, victim offset per preemptor; the victims
+    if (G) {
+        const size_t M = std::max<uint32_t>(m, 1);
+        CK(grow(e->prn_u32, 2 * M + 3 * (size_t)G + 2 + P)); CK(grow(e->prn_i32, M + P)); CK(grow(e->prn_room, (size_t)D * G));
+        for (int b = 0; b < 2; ++b) { CK(grow(e->prn_key[b], M)); CK(grow(e->prn_val[b], M)); }
+        CK(grow(e->prn_out, 3 * (size_t)P + M)); CK(grow(e->prn_taken, M));
+        size_t tb = 0;
+        CK(cub::DeviceRadixSort::SortPairs(nullptr, tb, e->prn_key[0].p, e->prn_key[1].p, e->prn_val[0].p, e->prn_val[1].p, (int)M, 0, 64, s));
+        CK(grow(e->prn_cub, tb));
+        uint32_t* d_sask = e->prn_u32.p; uint32_t* d_stg = d_sask + M; uint32_t* d_gnode = d_stg + M; uint32_t* d_gseg = d_gnode + G;
+        uint32_t* d_gpoff = d_gseg + G + 1; uint32_t* d_pask = d_gpoff + G + 1;
+        int32_t* d_sprio = e->prn_i32.p; int32_t* d_pprio = d_sprio + M;
+        uint32_t* d_st = e->prn_out.p; uint32_t* d_vout = d_st + 3 * (size_t)P;
+        CK(cudaMemcpyAsync(d_gnode, gnode.data(), 4 * (size_t)G, cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(d_gseg, gseg.data(), 4 * (size_t)(G + 1), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(d_gpoff, gpoff.data(), 4 * (size_t)(G + 1), cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(d_pask, pask.data(), 4 * (size_t)P, cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(d_pprio, pprio.data(), 4 * (size_t)P, cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(e->prn_room.p, room.data(), 8 * room.size(), cudaMemcpyHostToDevice, s));
+        e->st.h2d_bytes += 4 * (3 * (size_t)G + 2 + 2 * (size_t)P) + 8 * room.size();
+        YkPRNArgs ra{};
+        ra.D = D;
+        ra.s_ask = d_sask; ra.s_prio = d_sprio; ra.s_tg = d_stg; ra.m = (int)m;
+        ra.g_node = d_gnode; ra.g_seg = d_gseg; ra.g_poff = d_gpoff; ra.g_room = e->prn_room.p; ra.G = (int)G;
+        ra.p_ask = d_pask; ra.p_prio = d_pprio;
+        ra.total = e->d_total.p; ra.ldn = N; ra.taint = e->d_taint.p; ra.label = e->d_label.p; ra.flags = e->d_flags.p;
+        ra.a_req = e->d_areq.p; ra.a_tol = e->d_atol.p; ra.a_need = e->d_aneed.p; ra.a_deny = e->d_adeny.p; ra.lda = e->maxA;
+        if (m) {   // the create order, then the victim order inside each group's segment
+            std::vector<uint32_t> iota(m);
+            for (uint32_t i = 0; i < m; ++i) iota[i] = i;
+            CK(cudaMemcpyAsync(d_sask, sask.data(), 4 * (size_t)m, cudaMemcpyHostToDevice, s));
+            CK(cudaMemcpyAsync(d_stg, stg.data(), 4 * (size_t)m, cudaMemcpyHostToDevice, s));
+            CK(cudaMemcpyAsync(d_sprio, sprio.data(), 4 * (size_t)m, cudaMemcpyHostToDevice, s));
+            CK(cudaMemcpyAsync(e->prn_key[0].p, ckey.data(), 8 * (size_t)m, cudaMemcpyHostToDevice, s));
+            CK(cudaMemcpyAsync(e->prn_val[0].p, iota.data(), 4 * (size_t)m, cudaMemcpyHostToDevice, s));
+            e->st.h2d_bytes += 24 * (size_t)m;
+            size_t t1 = e->prn_cub.n;
+            CK(cub::DeviceRadixSort::SortPairs(e->prn_cub.p, t1, e->prn_key[0].p, e->prn_key[1].p, e->prn_val[0].p, e->prn_val[1].p, (int)m, 0, 64, s));
+            yk_prn_key_kernel<<<(m + 255) / 256, 256, 0, s>>>(ra, e->prn_val[1].p, e->prn_key[0].p, e->prn_val[0].p);
+            CK(cudaGetLastError());
+            t1 = e->prn_cub.n;
+            CK(cub::DeviceRadixSort::SortPairs(e->prn_cub.p, t1, e->prn_key[0].p, e->prn_key[1].p, e->prn_val[0].p, e->prn_val[1].p, (int)m, 0, 64, s));
+            e->st.other_launches += 10 + 1 + 10;   // two cub radix sorts of 64-bit keys and the key kernel
+        }
+        yk_prn_node_kernel<<<(G + 3) / 4, 128, 0, s>>>(ra, e->prn_val[1].p, e->prn_taken.p, d_st, d_st + P, d_st + 2 * (size_t)P, d_vout);
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(dst.data(), d_st, 4 * dst.size(), cudaMemcpyDeviceToHost, s));
+        if (m) CK(cudaMemcpyAsync(vout.data(), d_vout, 4 * (size_t)m, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        e->st.other_launches += 1;
+        e->st.d2h_bytes += 4 * (dst.size() + (size_t)m);
+    }
+
+    // ---- the caller-order prefix that fits victims_cap: mark and plan ----
+    uint32_t voff = 0, done = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t at = ppos[i];
+        const uint32_t st = at == YK_NONE ? status[i] : dst[at];
+        const uint32_t cnt = at == YK_NONE ? 0 : dst[P + at];
+        if (st == YK_PP_PLANNED && (uint64_t)voff + cnt > victims_cap) break;   // stops before this ask
+        status_out[i] = st;
+        victim_off_out[i] = voff;
+        if (st == YK_PP_PLANNED) {
+            for (uint32_t j = 0; j < cnt; ++j) {
+                const uint32_t v = vout[dst[2 * (size_t)P + at] + j];
+                victims_out[voff++] = v;
+                e->pp_mark[v] = 1;
+            }
+            e->pp_plan[asks[i]] = e->a_node[asks[i]];
+        }
+        done = i + 1;
+    }
     victim_off_out[done] = voff;
     *n_done = done;
     return YK_OK;

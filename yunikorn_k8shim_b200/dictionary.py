@@ -9,7 +9,7 @@ OPS = {"In": 0, "NotIn": 1, "Exists": 2, "DoesNotExist": 3, "Gt": 4, "Lt": 5}
 EFFECTS = {"": 0, "NoSchedule": 1, "PreferNoSchedule": 2, "NoExecute": 3}
 TOL_OPS = {"": 0, "Equal": 0, "Exists": 1}
 DICT_EXPORTS = ["yk_dict_create", "yk_dict_destroy", "yk_dict_node", "yk_dict_node_remove", "yk_dict_pod",
-                "yk_dict_generation", "yk_dict_node_bits"]
+                "yk_dict_pod_required_node", "yk_dict_generation", "yk_dict_node_bits"]
 
 
 class _Req(C.Structure):
@@ -106,23 +106,41 @@ class Dictionary:
         """affinity_terms: list of {"expr": [...], "fields": [...]} or None; has_affinity defaults to
         (affinity_terms is not None) -- pass has_affinity=True with affinity_terms=None for a nil term list."""
         keep = []
-        sel = node_selector or {}
-        ks, vs = _strs(list(sel.keys())), _strs(list(sel.values()))
-        terms = affinity_terms or []
-        if has_affinity is None:
-            has_affinity = affinity_terms is not None
-        ta = (_Term * max(len(terms), 1))()
-        for i, t in enumerate(terms):
-            ex, fl = t.get("expr") or [], t.get("fields") or []
-            ta[i] = _Term(len(ex), C.cast(_reqs(ex, keep), C.POINTER(_Req)), len(fl), C.cast(_reqs(fl, keep), C.POINTER(_Req)))
-        tols = tolerations or []
-        to = (_Tol * max(len(tols), 1))()
-        for i, t in enumerate(tols):
-            to[i] = _Tol(t.get("key", "").encode(), TOL_OPS[t.get("op", "")], t.get("value", "").encode(), EFFECTS[t.get("effect", "")])
-        spec = _PodSpec(len(sel), C.cast(ks, C.POINTER(C.c_char_p)), C.cast(vs, C.POINTER(C.c_char_p)),
-                        1 if has_affinity else 0, len(terms), ta, len(tols), to, (node_name or "").encode())
+        spec = _spec(keep, node_selector, affinity_terms, has_affinity, tolerations, node_name)
         out = PodMasks()
         rc = self._lib.yk_dict_pod(self._h, C.byref(spec), C.byref(out))
         if rc != 0:
             raise YkError(rc, "yk_dict_pod")
         return out
+
+    def pod_required_node(self, required_node, node_selector=None, affinity_terms=None, has_affinity=None, tolerations=None,
+                          node_name=None) -> PodMasks:
+        """a pod whose node is fixed (a DaemonSet pod): masks as pod(...) gives, with required_node = the index of the node
+        named required_node and the affinity terms resolved against that name"""
+        keep = []
+        spec = _spec(keep, node_selector, affinity_terms, has_affinity, tolerations, node_name)
+        out = PodMasks()
+        rc = self._lib.yk_dict_pod_required_node(self._h, C.byref(spec), required_node.encode(), C.byref(out))
+        if rc != 0:
+            raise YkError(rc, "yk_dict_pod_required_node")
+        return out
+
+
+def _spec(keep, node_selector, affinity_terms, has_affinity, tolerations, node_name):
+    sel = node_selector or {}
+    ks, vs = _strs(list(sel.keys())), _strs(list(sel.values()))
+    keep += [ks, vs]
+    terms = affinity_terms or []
+    if has_affinity is None:
+        has_affinity = affinity_terms is not None
+    ta = (_Term * max(len(terms), 1))()
+    for i, t in enumerate(terms):
+        ex, fl = t.get("expr") or [], t.get("fields") or []
+        ta[i] = _Term(len(ex), C.cast(_reqs(ex, keep), C.POINTER(_Req)), len(fl), C.cast(_reqs(fl, keep), C.POINTER(_Req)))
+    tols = tolerations or []
+    to = (_Tol * max(len(tols), 1))()
+    for i, t in enumerate(tols):
+        to[i] = _Tol(t.get("key", "").encode(), TOL_OPS[t.get("op", "")], t.get("value", "").encode(), EFFECTS[t.get("effect", "")])
+    keep += [ta, to]
+    return _PodSpec(len(sel), C.cast(ks, C.POINTER(C.c_char_p)), C.cast(vs, C.POINTER(C.c_char_p)),
+                    1 if has_affinity else 0, len(terms), ta, len(tols), to, (node_name or "").encode())

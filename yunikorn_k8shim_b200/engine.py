@@ -22,7 +22,7 @@ ASK_SLOWPATH = 1
 ASK_NO_PREEMPT_SELF = 2    # not AllowPreemptSelf
 ASK_NO_PREEMPT_OTHER = 4   # not AllowPreemptOther (preemptionPolicy: Never)
 ASK_ORIGINATOR = 8
-# yk_preemption_plan statuses
+# yk_preemption_plan and yk_preemption_required_node statuses
 PP_PLANNED, PP_FITS, PP_NOT_BLOCKED, PP_NOT_ALLOWED, PP_UNSUPPORTED, PP_GUARANTEE, PP_NO_VICTIMS = range(7)
 
 EXPORTS = [
@@ -31,7 +31,8 @@ EXPORTS = [
     "yk_asks_remove", "yk_release",
     "yk_asks_resize", "yk_cycle",
     "yk_ask_states", "yk_nodes_available", "yk_evaluate", "yk_evaluate_reserve", "yk_node_scores", "yk_node_sort_set", "yk_filter_nodes",
-    "yk_preemption_search", "yk_preemption_nodes", "yk_preemption_plan", "yk_set_exchange",
+    "yk_preemption_search", "yk_preemption_nodes", "yk_preemption_plan", "yk_preemption_required_node",
+    "yk_set_exchange",
     "yk_peer_export", "yk_peer_import", "yk_peer_enable", "yk_stats",
     "yk_stats_reset", "yk_strerror", "yk_last_error",
 ]
@@ -393,6 +394,22 @@ class Engine:
                                               _p(vic) if cap else None, C.c_uint32(cap), C.byref(done)))
         d = done.value
         return status[:d].copy(), node[:d].copy(), [vic[off[i]:off[i + 1]].copy() for i in range(d)], d
+
+    def preemption_required_node(self, asks, victims_cap=None):
+        """preemption for required-node (DaemonSet) asks on their own node, in order -> (status[d], victims: d arrays of ask
+        indices, d = n_done); victims_cap (default max_asks) bounds the victims of the whole call: planning stops before the
+        ask that would pass it"""
+        asks = _arr(asks, np.uint32)
+        n = asks.size
+        cap = self.max_asks if victims_cap is None else int(victims_cap)
+        status = np.zeros(max(n, 1), dtype=np.uint32)
+        off = np.zeros(n + 1, dtype=np.uint32)
+        vic = np.zeros(max(cap, 1), dtype=np.uint32)
+        done = C.c_uint32(0)
+        self._ck(self._lib.yk_preemption_required_node(self._h, C.c_uint32(n), _p(asks), _p(status), _p(off),
+                                                       _p(vic) if cap else None, C.c_uint32(cap), C.byref(done)))
+        d = done.value
+        return status[:d].copy(), [vic[off[i]:off[i + 1]].copy() for i in range(d)], d
 
     def set_exchange(self, fn):
         cb = ALLGATHER_FN(fn) if fn is not None else C.cast(None, ALLGATHER_FN)

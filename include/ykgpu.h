@@ -219,7 +219,14 @@ int yk_queues_priority(yk_engine* e, uint32_t q, const int32_t* offset, const ui
 int yk_queues_preemption(yk_engine* e, uint32_t q, const uint8_t* fence);
 
 /* applications live in LEAF queues (as in the core: placement into a parent queue is rejected there; here an application
- * whose queue has children is accepted but never scheduled -- the adapter must not produce one) */
+ * whose queue has children is accepted but never scheduled -- the adapter must not produce one).
+ * An application's allocations stay accounted to its index and its queue chain until each is released, even after
+ * yk_apps_remove; a removed application's index must not come back while any ask of it is still allocated.  So
+ * yk_apps_upsert returns YK_ERR_STATE and changes nothing when one of its entries
+ *   - names an index that is not present while an allocated ask still belongs to it (release those first), or
+ *   - moves a present application to another queue while an allocated ask belongs to it (its holdings would stay on
+ *     the old queue chain).
+ * An allocated ask counts as held whatever its request, zero included. */
 int yk_apps_upsert(yk_engine* e, uint32_t n, const uint32_t* idx, const uint32_t* queue,
                    const int64_t* submit_time);
 int yk_apps_remove(yk_engine* e, uint32_t n, const uint32_t* idx);

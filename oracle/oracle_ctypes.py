@@ -28,7 +28,7 @@ class _Snap(C.Structure):
         ("ask_flags", C.c_void_p), ("ask_gang", C.c_void_p),
         ("q_prio_offset", C.c_void_p), ("q_prio_fence", C.c_void_p),
         ("app_user", C.c_void_p), ("n_limits", C.c_int32), ("ul_queue", C.c_void_p), ("ul_user", C.c_void_p),
-        ("ul_max", C.c_void_p), ("ul_alloc", C.c_void_p),
+        ("ul_max", C.c_void_p), ("ul_alloc", C.c_void_p), ("app_alloc", C.c_void_p),
     ]
 
 
@@ -93,6 +93,8 @@ def _pack(s):
         st.ul_queue, st.ul_user = arr(s.ul_queue, np.int32), arr(s.ul_user, np.int32)
         st.ul_max = arr(s.ul_max, np.int64)
         st.ul_alloc = arr(s.ul_alloc, np.int64) if getattr(s, "ul_alloc", None) is not None else None
+    if getattr(s, "app_alloc", None) is not None:
+        st.app_alloc = arr(np.asarray(s.app_alloc, np.int64).reshape(s.n_apps, s.D), np.int64)
     return st, keep
 
 

@@ -97,7 +97,8 @@ def run(s, max_bindings=-1):
         app_asks[p].sort(key=lambda a: (-int(s.ask_prio[a]), int(s.ask_create[a]), a))
     state = [ST_PENDING] * A
     dead = [False] * A
-    app_alloc = [[0] * D for _ in range(s.n_apps)]
+    held = getattr(s, "app_alloc", None)      # what each application holds from earlier cycles (None = nothing)
+    app_alloc = [[int(x) for x in held[p]] if held is not None else [0] * D for p in range(s.n_apps)]
 
     def chain(q):
         while q >= 0:

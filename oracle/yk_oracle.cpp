@@ -552,7 +552,8 @@ int yko_run(const yko_snapshot* s, uint32_t mode, int32_t max_bindings, int32_t*
     for (int p = 0; p < s->n_apps; ++p) {
         if (!e.queues[(size_t)s->app_queue[p]].children.empty()) return -10;  // apps live in leaves
         e.queues[(size_t)s->app_queue[p]].apps.push_back(p);
-        e.apps[(size_t)p].alloc.assign((size_t)D, 0);
+        if (s->app_alloc) e.apps[(size_t)p].alloc.assign(s->app_alloc + (size_t)p * D, s->app_alloc + (size_t)(p + 1) * D);
+        else e.apps[(size_t)p].alloc.assign((size_t)D, 0);
         if (s->app_user && s->n_limits > 0 && s->app_user[p] >= 0)
             for (int l = 0; l < s->n_limits; ++l) {
                 if (s->ul_user[l] != s->app_user[p]) continue;

@@ -95,6 +95,8 @@ typedef struct {
     const int32_t* ul_user;         /* [l] */
     const int64_t* ul_max;          /* [l][D], -1 = not set */
     const int64_t* ul_alloc;        /* [l][D] held at cycle start; may be NULL = 0 */
+    /* what each application holds from earlier cycles: a fair leaf orders its applications by these shares */
+    const int64_t* app_alloc;       /* [p][D] held at cycle start; may be NULL = 0 */
 } yko_snapshot;
 
 typedef struct {

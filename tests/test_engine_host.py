@@ -64,6 +64,11 @@ def run_engine_host(shim, s, batch=256, epoch_limit=None, speculate=1, max_bindi
             setter(_p(k["puser"]), C.c_uint32(len(s.ul_queue)), _p(k["ulq"]), _p(k["ulu"]), _p(k["ulm"]), _p(k["ula"]))
         else:
             setter(None, C.c_uint32(0), None, None, None, None)
+    setter = getattr(shim, "host_set_app_alloc", None)
+    if setter is not None:
+        held = getattr(s, "app_alloc", None)
+        k["palloc"] = np.ascontiguousarray(np.asarray(held, dtype=np.int64).reshape(P, D).T) if held is not None else None
+        setter(_p(k["palloc"]) if held is not None else None)
     out_ask = np.zeros(max(A, 1), dtype=np.uint32)
     out_node = np.zeros(max(A, 1), dtype=np.uint32)
     n = C.c_uint32(0)

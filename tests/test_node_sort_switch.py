@@ -9,8 +9,8 @@ setting and loaded with the same tables would be in.
 The sessions are test_sessions' Model / Generator with one more operation between cycles: a switch of policy and weights
 (default, all zero, configured, or weighting a resource on which some nodes have total 0 and so an infinite share).  The
 model passes its current policy and weights to the oracle every cycle and the engine gets the same node_sort_set call, so
-test_sessions.replay checks every cycle of a switched session exactly as it checks an unswitched one.  Leaves stay fifo for
-the reason test_sessions states.  The CPU tests check that both oracles agree on every switched cycle and that the sessions
+test_sessions.replay checks every cycle of a switched session exactly as it checks an unswitched one.  Sessions with a
+seed of at least test_sessions.MIXED_FROM have fair leaves too.  The CPU tests check that both oracles agree on every switched cycle and that the sessions
 switch in every direction and with every kind of weights."""
 import copy
 import ctypes as C
@@ -74,7 +74,7 @@ def switched_session(oracle, seed, D=4, policy=FAIR):
     m = ts.Model(oracle, f"switched(seed={seed}, D={D}, policy={policy})", D, policy, max_nodes=128, max_asks=1024,
                  seed=seed + 1000 * D)
     m.initial = (policy, m.weights.copy())
-    g = ts.Generator(m, rng)
+    g = ts.Generator(m, rng, leaves=ts.leaves(seed))
     g.start(int(rng.integers(12, 40)))
     for c in range(int(rng.integers(14, 27))):
         if c:
@@ -89,7 +89,8 @@ def switched_session(oracle, seed, D=4, policy=FAIR):
 
 
 SWITCHED = [(s, 4, FAIR) for s in range(5)] + [(s, 4, BP) for s in range(5, 10)] \
-    + [(10, 1, FAIR), (11, 1, BP), (12, 8, FAIR), (13, 8, BP)]
+    + [(10, 1, FAIR), (11, 1, BP), (12, 8, FAIR), (13, 8, BP)] \
+    + [(200, 4, FAIR), (201, 4, BP)]                                   # fair leaves (ts.MIXED_FROM)
 SWITCHED_IDS = [f"seed{s}-D{d}-{NAMES[p]}" for s, d, p in SWITCHED]
 
 

@@ -221,7 +221,7 @@ def resized_session(oracle, seed, D=4, policy=FAIR):
     m = ts.Model(oracle, f"resized(seed={seed}, D={D}, policy={policy})", D, policy, max_nodes=128, max_asks=1024,
                  seed=seed + 1000 * D)
     m.initial = (policy, m.weights.copy())
-    g = ts.Generator(m, rng)
+    g = ts.Generator(m, rng, leaves=ts.leaves(seed))
     g.start(int(rng.integers(12, 40)))
     for c in range(int(rng.integers(14, 27))):
         if c:
@@ -237,7 +237,8 @@ def resized_session(oracle, seed, D=4, policy=FAIR):
 
 
 RESIZED = [(s, 4, FAIR) for s in range(5)] + [(s, 4, BP) for s in range(5, 8)] \
-    + [(8, 1, FAIR), (9, 1, BP), (10, 8, FAIR), (11, 8, BP)]
+    + [(8, 1, FAIR), (9, 1, BP), (10, 8, FAIR), (11, 8, BP)] \
+    + [(200, 4, FAIR), (201, 4, BP), (202, 1, FAIR), (203, 8, FAIR)]   # fair leaves (ts.MIXED_FROM)
 RESIZED_IDS = [f"seed{s}-D{d}-{tns.NAMES[p]}" for s, d, p in RESIZED]
 
 
@@ -327,8 +328,32 @@ def t_overcommit(oracle, path):
     return m
 
 
+def t_fair_resize(oracle):
+    """resizes decide a fair leaf's next order: applications 0, 1, 2 hold alike, so submit time orders them; 2's allocations
+    grow and it goes last; then 0's shrink to zero on every resource (still held) and 1's grow past 2's: 0 goes first,
+    then 2 before 1"""
+    m = ts._fair_base(oracle, "fair-resize-order", 12, apps=(3, 3, 3))
+    for p in range(3):
+        m.asks_upsert(list(range(4 * p, 4 * p + 4)), ts._req(1000), p)
+    m.cycle()
+    resize(m, [8, 9], np.stack([ts._req(3000, 2 * GI)] * 2))
+    for p in range(3):
+        m.asks_upsert([20 + 2 * p, 21 + 2 * p], ts._req(200), p)
+    ask, _, _ = m.cycle(5)
+    assert [int(m.a_app[a]) for a in ask] == [0, 1, 0, 1, 2], ask
+    resize(m, [0, 1, 2, 3], np.zeros((4, 4), np.int64))
+    resize(m, [4, 5, 6, 7], np.stack([ts._req(4000, 4 * GI)] * 4))
+    for p in range(3):
+        m.asks_upsert([30 + 2 * p, 31 + 2 * p], ts._req(200), p)
+    ask, _, _ = m.cycle(6)
+    assert [int(m.a_app[a]) for a in ask][:4] == [0, 0, 2, 2] and ts.history_decided(m, ts._cycles(m)[-1]), ask
+    ts.finish(m)
+    return m
+
+
 TARGETED = {"resize": t_resize, "overcommit_uniform": lambda o: t_overcommit(o, "uniform"),
-            "overcommit_rounds": lambda o: t_overcommit(o, "rounds"), "overcommit_fill": lambda o: t_overcommit(o, "fill")}
+            "overcommit_rounds": lambda o: t_overcommit(o, "rounds"), "overcommit_fill": lambda o: t_overcommit(o, "fill"),
+            "fair_resize": t_fair_resize}
 
 
 # ---- GPU: 1. resized sessions ----
@@ -344,6 +369,13 @@ def test_resized_session(monkeypatch, seed, D, policy, commit, batch, bp_device)
     _, tot = tns.replay(monkeypatch, m, commit, batch, bp_device, filter_k=9 if commit == "host" and batch == 64 else None)
     if commit == "device" and (policy == FAIR or bp_device):
         assert tot["lattice_cycles"] > 0, m.name
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("commit", ["host", "device", "auto"])
+def test_fair_resize_script(oracle, monkeypatch, commit):
+    """resized holdings decide a fair leaf's order on every commit"""
+    tns.replay(monkeypatch, t_fair_resize(oracle), commit, 64, False)
 
 
 # ---- GPU: 2. a resized engine equals a fresh one ----

@@ -15,7 +15,14 @@ snapshot, the accounting is conserved after every step, and the generated sessio
 
 NodeIDs are zero-padded numbers (`n000123`) and the rank given to yk_nodes_upsert is that number: sparse and
 order-preserving.  Create sequence numbers and submit times are unique, so compacting cannot reorder ties.
-Removing an application that still holds allocations is not defined by include/ykgpu.h and is never generated."""
+The generator never removes an application that still holds allocations; the targeted script `n_refused_upsert` does, and
+checks that its index cannot come back (yk_apps_upsert refuses it) until they are released.
+
+Leaves are fifo by default.  Sessions with a seed of at least MIXED_FROM draw every leaf fifo or fair at every queues_set
+(at least one fair, 2-4 applications in each, guarantees unset, set on some resources or 0): a fair leaf orders its
+applications by what each already holds, so the model's snapshot then carries every application's holdings (app_alloc),
+and a cycle is history-decided when the oracle's bindings change once those are zeroed."""
+import copy
 import functools
 
 import numpy as np
@@ -23,9 +30,12 @@ import pytest
 
 from yunikorn_k8shim_b200 import synth
 from oracle import py_oracle
+from device_shim import dshim  # noqa: F401  (fixtures)
+from test_engine_host import shim  # noqa: F401
 
 GI = synth.GI
 ABSENT, PENDING, ALLOCATED, NOFIT = 255, 0, 1, 2
+YK_ERR_STATE = -4
 SCHED, RESERVED = synth.NODE_SCHEDULABLE, synth.NODE_RESERVED
 # root -> two parents -> three leaves (leaves 3 and 4 under parent 1, leaf 5 under parent 2); applications live in leaves
 Q_PARENT = np.array([-1, 0, 0, 1, 1, 2], dtype=np.int32)
@@ -94,6 +104,8 @@ class Model:
         self.cycles = 0
         self.since = []                                 # op texts since the last cycle
         self.removed_below_hi = False
+        self.gone_holding = set()                       # removed applications that still hold allocations
+        self.initial = (policy, self.weights.copy())    # the node sort an engine for the script is created with
 
     # ---- bookkeeping ----
     def note(self, key, n=1):
@@ -128,6 +140,17 @@ class Model:
             for q in self.chain(self.p_queue[self.a_app[a]]):
                 qa[q] += self.a_req[a]
         return qa
+
+    def app_alloc(self):
+        """[P][D] what each application's allocated asks hold (on removed nodes too)"""
+        pa = np.zeros((self.maxP, self.D), np.int64)
+        for a in np.nonzero(self.a_state == ALLOCATED)[0]:
+            pa[self.a_app[a]] += self.a_req[a]
+        return pa
+
+    def holds(self, p):
+        """whether an allocated ask belongs to application p (whatever its request, zero included)"""
+        return bool(((self.a_app == p) & (self.a_state == ALLOCATED)).any())
 
     def held(self):
         h = np.zeros((len(self.ul), self.D), np.int64)
@@ -197,14 +220,28 @@ class Model:
         self._op("apps_upsert", "apps_upsert", idx=idx, queue=queue, submit_time=submit)
         self._op("apps_user", "apps_user", idx=idx, user=user)
 
-    def apps_remove(self, idx):
+    def apps_remove(self, idx, holding=False):
+        """holding: the application may keep allocations; they stay on its index and queue chain until released"""
         idx = np.atleast_1d(np.asarray(idx, np.int64))
         for p in idx:
-            assert not ((self.a_app == p) & (self.a_state == ALLOCATED)).any(), "an application with allocations"
+            assert holding or not self.holds(p), "an application with allocations"
+            if self.holds(p):
+                self.gone_holding.add(int(p))
+                self.note("app_removed_holding")
             if ((self.a_app == p) & (self.a_state == PENDING)).any():
                 self.note("app_removed_with_pending")
             self.p_present[p] = False
         self._op("apps_remove", "apps_remove", idx=idx)
+
+    def apps_upsert_refused(self, idx, queue):
+        """a yk_apps_upsert the engine must refuse with YK_ERR_STATE and nothing changed: an index that comes back while
+        allocations of it are held, or a present application moved to another queue while it holds allocations"""
+        idx = np.atleast_1d(np.asarray(idx, np.int64))
+        queue = np.broadcast_to(np.asarray(queue, np.int64), idx.shape).copy()
+        assert any(self.holds(p) and (not self.p_present[p] or self.p_queue[p] != q) for p, q in zip(idx, queue))
+        self.note("apps_upsert_refused")
+        self.steps.append(("refused", "apps_upsert", dict(idx=idx, queue=queue, submit_time=np.full(len(idx), 1_600_000_000)),
+                           "apps_upsert(refused)"))
 
     def asks_upsert(self, idx, req, app, tol=0, need=0, deny=0, prio=0, flags=0, gang=-1, text="asks_upsert"):
         idx = np.atleast_1d(np.asarray(idx, np.int64))
@@ -245,9 +282,16 @@ class Model:
             self.a_state[a], self.a_bound[a] = ABSENT, -1   # index is never reused while an allocation points at it
             if self.a_gang[a] >= 0:
                 self.note("release_gang_member")
+        self.gone_holding = {p for p in self.gone_holding if self.holds(p)}
         self._op("release", text, ask_idx=idx)
 
     def queues_set(self, guar, mx, sort):
+        sort = np.asarray(sort, np.uint8)
+        leaves = list(LEAVES)
+        if (self.q_sort[leaves] < sort[leaves]).any():
+            self.since.append("leaf_fifo_to_fair")
+        if sort[leaves].any() and not np.array_equal(self.q_guar[leaves], np.asarray(guar, np.int64)[leaves]):
+            self.since.append("guarantee_change")
         self.q_guar, self.q_max, self.q_sort = np.asarray(guar, np.int64), np.asarray(mx, np.int64), np.asarray(sort, np.uint8)
         self.q_prio_offset = self.q_prio_fence = None     # yk_queues_set resets the priority properties
         self._op("queues_set", "queues_set", parent=Q_PARENT.copy(), guaranteed=self.q_guar.copy(), max=self.q_max.copy(),
@@ -288,6 +332,8 @@ class Model:
             ask_gang=self.a_gang[asks].astype(np.int32), name=f"{self.name}-c{self.cycles}",
             q_prio_offset=None if self.q_prio_offset is None else self.q_prio_offset.copy(),
             q_prio_fence=None if self.q_prio_fence is None else self.q_prio_fence.copy())
+        if (self.q_sort[list(LEAVES)] == 1).any():   # all-fifo snapshots stay without: no order reads it
+            s.app_alloc = self.app_alloc()[apps]
         if self.ul:
             s.app_user = self.p_user[apps].astype(np.int32)
             s.ul_queue = np.array([e[0] for e in self.ul], np.int32)
@@ -344,7 +390,7 @@ class Model:
         """what the model's allocations hold is exactly what the nodes, queues and users account for"""
         used = np.zeros_like(self.n_used)
         for a in np.nonzero(self.a_state == ALLOCATED)[0]:
-            assert self.a_bound[a] >= 0 and self.p_present[self.a_app[a]], (self.name, int(a))
+            assert self.a_bound[a] >= 0 and (self.p_present[self.a_app[a]] or int(self.a_app[a]) in self.gone_holding), (self.name, int(a))
             used[self.a_bound[a]] += self.a_req[a]
         assert np.array_equal(used, self.n_used), self.name
         qa = self.q_alloc()
@@ -422,8 +468,14 @@ def _random_node(m, n, rng, tied_shape=None):
 
 
 class Generator:
-    def __init__(self, m, rng, big=0):
-        self.m, self.rng, self.big = m, rng, big
+    def __init__(self, m, rng, big=0, leaves="fifo"):
+        """leaves: "fifo" (every leaf fifo), or "mixed" (each leaf fifo or fair, drawn at every queues_set)"""
+        assert leaves in ("fifo", "mixed")
+        self.m, self.rng, self.big, self.mixed = m, rng, big, leaves == "mixed"
+
+    def leaf_apps(self, q):
+        m = self.m
+        return [int(p) for p in np.nonzero(m.p_present)[0] if m.p_queue[p] == q]
 
     # nodes
     def add_nodes(self, k, tied=False):
@@ -555,6 +607,23 @@ class Generator:
                 m.asks_upsert(idx, req, p, tol, need, deny, prio, flags=flags)
                 m.note("asks_new")
 
+    def twin_asks(self):
+        """two applications of one leaf get the same asks: once both are placed they hold equal amounts, and a fair leaf
+        orders them by submit time, then index"""
+        m, rng = self.m, self.rng
+        leaves = [q for q in LEAVES if len(self.leaf_apps(q)) >= 2]
+        if not leaves:
+            return
+        pair = rng.choice(self.leaf_apps(int(rng.choice(leaves))), 2, replace=False)
+        req, k = _ask_shape(rng, m.D), int(rng.integers(1, 4))
+        if not req.any():
+            req[0] = 100
+        for p in sorted(pair.tolist()):
+            idx = self.ask_indices(k)
+            if idx:
+                m.asks_upsert(idx, req, p, np.uint64(7), text="asks_upsert(twin)")
+        m.note("asks_twin")
+
     def reupsert_asks(self):
         m, rng = self.m, self.rng
         cand = [a for a in np.nonzero(m.a_state == PENDING)[0] if m.a_gang[a] < 0 and m.p_present[m.a_app[a]]]
@@ -595,13 +664,20 @@ class Generator:
         m, rng = self.m, self.rng
         live = set(m.a_app[:m.a_hi][m.a_state[:m.a_hi] != ABSENT].tolist())
         free = [p for p in range(m.maxP) if not m.p_present[p] and p not in live]
-        if free:
+        if free and self.mixed:                        # the leaf with the fewest applications, never more than 4
+            q = min(LEAVES, key=lambda x: len(self.leaf_apps(x)))
+            if len(self.leaf_apps(q)) < 4:
+                m.apps_upsert([free[0]], q, int(rng.integers(-1, 3)))
+                m.note("apps_upsert")
+        elif free:
             m.apps_upsert([free[0]], int(rng.choice(LEAVES)), int(rng.integers(-1, 3)))
             m.note("apps_upsert")
 
     def remove_app(self):
         m, rng = self.m, self.rng
         cand = [p for p in np.nonzero(m.p_present)[0] if not ((m.a_app == p) & (m.a_state == ALLOCATED)).any()]
+        if self.mixed:                                 # every leaf keeps at least 2
+            cand = [p for p in cand if len(self.leaf_apps(m.p_queue[p])) > 2]
         if len(np.nonzero(m.p_present)[0]) <= 2 or not cand:
             return
         p = int(rng.choice(cand))
@@ -622,9 +698,28 @@ class Generator:
                 mx[q, 0] = int(rng.integers(3, 40)) * 1000
             if m.D > 2 and rng.random() < 0.15:
                 mx[q, 2] = int(rng.integers(5, 40))
-        # fifo leaves only: a fair leaf orders its applications by what each has held since earlier cycles, and the oracle's
-        # snapshot has no per-application allocation to start from (it would start every application at zero)
-        m.queues_set(guar, mx, np.zeros(m.maxQ, np.uint8))
+        sort = np.zeros(m.maxQ, np.uint8)
+        if self.mixed:
+            sort[list(LEAVES)] = rng.random(len(LEAVES)) < 0.6
+            if not sort.any():
+                sort[int(rng.choice(LEAVES))] = 1
+            for q in LEAVES:                           # a fair leaf's guarantee: unset, on some resources, or 0 on one
+                kind = int(rng.integers(0, 3))
+                guar[q] = -1
+                if kind == 1:
+                    for k in range(m.D):
+                        if rng.random() < 0.6:
+                            guar[q, k] = max(1, int(_node_shape(rng, m.D)[k]) * int(rng.integers(1, 4)))
+                elif kind == 2:
+                    guar[q, int(rng.integers(0, m.D))] = 0
+                    if m.D > 1:
+                        guar[q, 0] = max(guar[q, 0], int(rng.integers(1, 20)) * 1000)
+            old = m.q_sort[list(LEAVES)]
+            if not first and (old > sort[list(LEAVES)]).any():
+                m.note("leaf_fair_to_fifo")
+            if not first and (old < sort[list(LEAVES)]).any():
+                m.note("leaf_fifo_to_fair")
+        m.queues_set(guar, mx, sort)
         if not first:
             m.note("queues_set")
 
@@ -691,6 +786,8 @@ class Generator:
             (0.05, self.priorities),
             (0.07, self.limits),
         ]
+        if self.mixed:
+            ops.append((0.3, self.twin_asks))
         if rng.random() < 0.12:                        # a release, and nothing else, before the cycle
             self.release()
             return
@@ -701,6 +798,8 @@ class Generator:
     def start(self, n_nodes, n_apps=4):
         m, rng = self.m, self.rng
         self.queues(first=True)
+        if self.mixed:
+            n_apps = 9
         m.apps_upsert(list(range(n_apps)), [LEAVES[i % 3] for i in range(n_apps)], [i % 3 - (i == 3) for i in range(n_apps)])
         tied = int(rng.integers(3, 7))
         shape = _node_shape(rng, m.D)
@@ -717,7 +816,7 @@ def random_session(oracle, seed, D=4, policy=synth.POLICY_FAIR, big=0):
     rng = np.random.default_rng([seed, D, policy, big])
     m = Model(oracle, f"session(seed={seed}, D={D}, policy={policy}, big={big})", D, policy,
               max_nodes=(big + 160) if big else 128, max_asks=1024, seed=seed + 1000 * D)
-    g = Generator(m, rng, big)
+    g = Generator(m, rng, big, leaves(seed))
     g.start(big - 10 if big else int(rng.integers(12, 40)))
     n_cycles = int(rng.integers(12, 31))
     for c in range(n_cycles):
@@ -742,11 +841,22 @@ def finish(m):
     m.check_conservation()
 
 
+MIXED_FROM = 200     # sessions with a seed from here on have fifo and fair leaves (Generator leaves="mixed")
+
+
+def leaves(seed):
+    return "mixed" if seed >= MIXED_FROM else "fifo"
+
+
 SEEDS = range(20)
 EXTRA = [(s, 1, synth.POLICY_FAIR, 0) for s in (100, 101)] + [(s, 8, synth.POLICY_FAIR, 0) for s in (102, 103)] \
     + [(s, 4, synth.POLICY_BINPACKING, 0) for s in (104, 105, 106)]
 BIG = [(110, 4, synth.POLICY_FAIR, 256), (111, 4, synth.POLICY_FAIR, 512)]
 ALL = [(s, 4, synth.POLICY_FAIR, 0) for s in SEEDS] + EXTRA + BIG
+# fair leaves: D = 1, 4, 8 under both node sorts, each replayed with and without the binpacking flag
+MIXED = [(MIXED_FROM + i, D, p, 0) for i, (D, p) in enumerate((D, p) for D in (1, 4, 8)
+                                                              for p in (synth.POLICY_FAIR, synth.POLICY_BINPACKING))]
+MIXED_PARITY = [(seed, D, p, bp) for seed, D, p, _ in MIXED for bp in (False, True)]
 
 
 @functools.lru_cache(maxsize=None)
@@ -784,6 +894,13 @@ def replay(m, commit="host", batch=64, filter_k=None, on_cycle=None):
             if step[0] == "op":
                 _, method, kw, _text = step
                 getattr(e, method)(**kw)
+                continue
+            if step[0] == "refused":
+                from yunikorn_k8shim_b200.engine import YkError
+                _, method, kw, _text = step
+                with pytest.raises(YkError) as err:
+                    getattr(e, method)(**kw)
+                assert err.value.code == YK_ERR_STATE, f"{m.name}: {_text}: {err.value}"
                 continue
             if step[0] == "conserved":
                 pres = m.present_nodes()
@@ -842,10 +959,17 @@ def _filter_check(e, m, c, k, where):
 @pytest.mark.gpu
 @pytest.mark.parametrize("batch", [7, 64, 4096])
 @pytest.mark.parametrize("commit", ["host", "device", "auto"])
-@pytest.mark.parametrize("seed", SEEDS)
+@pytest.mark.parametrize("seed", list(SEEDS) + MIXED_PARITY,
+                         ids=lambda x: None if isinstance(x, int) else f"fairleaves{x[0]}-D{x[1]}-p{x[2]}-{'bpdevice' if x[3] else 'noflag'}")
 def test_session_parity(monkeypatch, seed, commit, batch):
+    """fifo sessions (an integer seed), and sessions with fair leaves: (seed, D, node sort, binpacking flag)"""
     monkeypatch.setenv("YK_UNIFORM_MIN", str(UNIFORM_MIN))
-    replay(session(seed), commit, batch)
+    if isinstance(seed, int):
+        replay(session(seed), commit, batch)
+        return
+    import test_node_sort_switch as tns
+    seed, D, policy, bp_device = seed
+    tns.replay(monkeypatch, session(seed, D, policy), commit, batch, bp_device)
 
 
 @pytest.mark.gpu
@@ -1053,8 +1177,160 @@ def t_quota_from_history(oracle):
     return m
 
 
+# ---- targeted sessions with fair leaves ----
+def _fair_base(oracle, name, n_nodes=12, guar=None, sort=(1, 0, 0), apps=(3, 3), **kw):
+    """_base with leaves 3, 4, 5 sorted as `sort` (1 = fair), leaf 3's guarantee `guar`, and applications 0, 1, ... in
+    `apps`' leaves"""
+    m = _base(oracle, name, n_nodes, apps=0, **kw)
+    g = np.full((m.maxQ, m.D), -1)
+    if guar is not None:
+        g[3] = guar
+    q_sort = np.zeros(m.maxQ, np.uint8)
+    q_sort[list(LEAVES)] = sort
+    m.queues_set(g, np.full((m.maxQ, m.D), -1), q_sort)
+    m.apps_upsert(list(range(len(apps))), list(apps))
+    return m
+
+
+def t_fair_flip(oracle):
+    """(i) a fifo leaf through a cycle on the uniform-run path and a cycle of mixed requests, both
+    placement-insensitive: the orderer's finish() keeps the holdings on its delta path.  Then queues_set makes the leaf fair,
+    and the next order is the holdings' order (application 0 holds more, application 1 goes first)"""
+    m = _fair_base(oracle, "fair-flip-after-device", 16, sort=(0, 0, 0))
+    m.asks_upsert(list(range(3 * UNIFORM_MIN)), _req(500), 0)
+    m.cycle()
+    m.asks_upsert(list(range(100, 140)), np.stack([_req(100 * (1 + i % 4), (256 << 20) * (1 + i % 2)) for i in range(40)]), 1)
+    m.cycle()
+    sort = np.zeros(m.maxQ, np.uint8)
+    sort[3] = 1
+    m.queues_set(m.q_guar, m.q_max, sort)
+    m.asks_upsert(list(range(200, 204)), _req(300), 0)
+    m.asks_upsert(list(range(204, 208)), _req(300), 1)
+    ask, _, _ = m.cycle(5)
+    assert m.a_app[ask[0]] == 1 and history_decided(m, _cycles(m)[-1])
+    finish(m)
+    return m
+
+
+def t_fair_release(oracle):
+    """(j) releases decide the next order: applications 0, 1, 2 hold 12, 8 and 4 asks' worth, so 2 goes first; then 1 gives
+    most of its holdings back, drops below 2 and goes first (from zero the order would be 0, 1, 2)"""
+    m = _fair_base(oracle, "fair-release-order", 12, guar=[4000, 8 * GI, -1, -1], apps=(3, 3, 3))
+    m.asks_upsert(list(range(12)), _req(1000), 0)
+    m.asks_upsert(list(range(12, 20)), _req(1000), 1)
+    m.asks_upsert(list(range(20, 24)), _req(1000), 2)
+    m.cycle()
+    for p in range(3):
+        m.asks_upsert([30 + 2 * p, 31 + 2 * p], _req(200), p)
+    ask, _, _ = m.cycle(1)
+    assert m.a_app[ask[0]] == 2 and history_decided(m, _cycles(m)[-1])
+    m.release(list(range(12, 18)))
+    ask, _, _ = m.cycle(1)
+    assert m.a_app[ask[0]] == 1 and history_decided(m, _cycles(m)[-1])
+    m.cycle()
+    finish(m)
+    return m
+
+
+def t_fair_nofit(oracle):
+    """(k) a NOFIT in a fair leaf: application 1 holds less, its first ask fits nowhere (on the device commit the lattice
+    kernel stops there and the batch is rewound to the application state it began with), its sibling's asks follow"""
+    m = _fair_base(oracle, "fair-nofit", 6, shape=np.array([4000, 16 * GI, 20, 4000]))
+    m.asks_upsert(list(range(6)), _req(1500), 0)
+    m.asks_upsert([6], _req(500), 1)
+    m.cycle()
+    m.asks_upsert([10], _req(3900), 1)                                 # fits no node: each has 2 500 left at most
+    m.asks_upsert(list(range(11, 15)), _req(600), 1)
+    m.asks_upsert(list(range(20, 26)), _req(700), 0)
+    m.cycle()
+    assert m.a_last[10] == NOFIT and history_decided(m, _cycles(m)[-1])
+    finish(m)
+    return m
+
+
+def t_fair_reused_index(oracle):
+    """(l) an application that held allocations releases them, is removed and its index comes back: it starts at zero and
+    goes before a sibling that holds something"""
+    m = _fair_base(oracle, "fair-reused-index", 10, apps=(3, 3, 3))
+    m.asks_upsert(list(range(6)), _req(1000), 2)
+    m.asks_upsert(list(range(6, 8)), _req(500), 1)
+    m.cycle()
+    m.release(list(range(6)))
+    m.apps_remove([2])
+    m.apps_upsert([2], 3)
+    m.asks_upsert(list(range(10, 13)), _req(400), 2)
+    m.asks_upsert(list(range(13, 16)), _req(400), 1)
+    m.asks_upsert(list(range(16, 19)), _req(400), 0)
+    ask, _, _ = m.cycle(2)
+    assert [int(m.a_app[a]) for a in ask] == [0, 2], ask
+    m.cycle()
+    finish(m)
+    return m
+
+
+def t_fair_rounding_tie(oracle):
+    """(m) holdings of 2^53 and 2^53 + 1 in a leaf without a guarantee: both shares are the same double, so the order falls
+    to submit time (application 1, upserted first), not to the larger holding"""
+    big = 1 << 53
+    m = _base(oracle, "fair-rounding-tie", 4, D=1, shape=np.array([1 << 55]), apps=0)
+    sort = np.zeros(m.maxQ, np.uint8)
+    sort[3] = 1
+    m.queues_set(np.full((m.maxQ, 1), -1), np.full((m.maxQ, 1), -1), sort)
+    m.apps_upsert([1], 3)
+    m.apps_upsert([0], 3)
+    m.asks_upsert([0], np.array([big + 1]), 1)
+    m.asks_upsert([1], np.array([big]), 0)
+    m.cycle()
+    assert float(big) == float(big + 1)
+    m.asks_upsert([2], np.array([7]), 0)
+    m.asks_upsert([3], np.array([7]), 1)
+    ask, _, _ = m.cycle(1)
+    assert ask.tolist() == [3], ask
+    m.cycle()
+    finish(m)
+    return m
+
+
+def t_refused_upsert(oracle):
+    """(n) yk_apps_upsert refuses, and changes nothing, (1) for an index that comes back while allocations of its removed
+    application are held, (2) for a present application moved to another queue while it holds allocations, one of them
+    resized to zero.  The next cycles equal those of an engine that never got the call; once the removed application's
+    allocations are released every queue, user entry and node is back at the oracle's values"""
+    m = _fair_base(oracle, "refused-upsert", 10, guar=[6000, -1, -1, -1], apps=(3, 3, 4))
+    m.p_user[:3] = [0, 1, 1]
+    m._op("apps_user", "apps_user", idx=np.arange(3), user=m.p_user[:3].copy())
+    m.user_limits_set([(1, 1, np.array([20000, -1, -1, -1]))])
+    m.asks_upsert(list(range(4)), _req(1000), 0)
+    m.asks_upsert(list(range(4, 10)), _req(1000), 1)
+    m.asks_upsert(list(range(10, 12)), _req(500), 2)
+    m.cycle()
+    m.apps_remove([1], holding=True)
+    m.apps_upsert_refused([1], 3)                                      # (1) the index comes back, same leaf
+    m.apps_upsert_refused([1], 4)                                      # (1) another leaf
+    m.asks_upsert(list(range(20, 24)), _req(700), 0)
+    m.asks_upsert(list(range(24, 28)), _req(700), 2)
+    m.cycle()
+    m.apps_upsert_refused([0], 5)                                      # (2) application 0 to another leaf
+    m.apps_upsert_refused([2, 0], [4, 4])                              # (2) in a call whose first entry is fine
+    import test_resize
+    held = [int(a) for a in np.nonzero((m.a_app == 2) & (m.a_state == ALLOCATED))[0]]
+    test_resize.resize(m, held, np.zeros((len(held), m.D), np.int64))   # application 2 holds allocations of nothing
+    assert held and not m.app_alloc()[2].any()
+    m.apps_upsert_refused([2], 5)
+    m.asks_upsert(list(range(28, 30)), _req(300), 0)
+    m.cycle()
+    m.release([a for a in range(4, 10) if m.a_state[a] == ALLOCATED])  # the removed application's allocations
+    m.apps_upsert([1], 4)                                              # now the index may come back, anywhere
+    m.asks_upsert(list(range(30, 34)), _req(600), 1)
+    m.cycle()
+    finish(m)
+    return m
+
+
 @pytest.mark.parametrize("name", sorted(["a_release_then_cycle", "b_removed_below_hi", "c_rename_tied", "d_nofit_then_fit",
-                                         "e_epoch_rows", "f_uniform_uneven", "g_gang_handoff", "h_quota_from_history"]))
+                                         "e_epoch_rows", "f_uniform_uneven", "g_gang_handoff", "h_quota_from_history",
+                                         "i_fair_flip", "j_fair_release", "k_fair_nofit", "l_fair_reused_index",
+                                         "m_fair_rounding_tie", "n_refused_upsert"]))
 def test_targeted_script(oracle, name):
     """each targeted script on the CPU: it has the shape it is meant to exercise (asserted inside), the model's accounting is
     conserved, and both oracles agree on every cycle"""
@@ -1065,11 +1341,14 @@ def test_targeted_script(oracle, name):
 
 TARGETED = {"a_release_then_cycle": t_release_then_cycle, "b_removed_below_hi": t_removed_below_hi,
             "c_rename_tied": t_rename_tied, "d_nofit_then_fit": t_nofit_then_fit, "e_epoch_rows": t_epoch_rows,
-            "f_uniform_uneven": t_uniform_uneven, "g_gang_handoff": t_gang_handoff, "h_quota_from_history": t_quota_from_history}
+            "f_uniform_uneven": t_uniform_uneven, "g_gang_handoff": t_gang_handoff, "h_quota_from_history": t_quota_from_history,
+            "i_fair_flip": t_fair_flip, "j_fair_release": t_fair_release, "k_fair_nofit": t_fair_nofit,
+            "l_fair_reused_index": t_fair_reused_index, "m_fair_rounding_tie": t_fair_rounding_tie,
+            "n_refused_upsert": t_refused_upsert}
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("commit", ["host", "device"])
+@pytest.mark.parametrize("commit", ["host", "device", "auto"])
 @pytest.mark.parametrize("name", sorted(TARGETED))
 def test_targeted_session(oracle, monkeypatch, name, commit):
     monkeypatch.setenv("YK_UNIFORM_MIN", str(UNIFORM_MIN))
@@ -1079,8 +1358,12 @@ def test_targeted_session(oracle, monkeypatch, name, commit):
     cyc = _cycles(m)
     if commit == "device":
         assert [d["lattice_cycles"] for d in per] == [int(c.eligible) for c in cyc], name
-    else:
+    elif commit == "host":
         assert all(d["lattice_cycles"] == 0 for d in per) and tot["sweep_launches"] > 0, name
+    if name == "i_fair_flip" and commit == "device":   # the fifo run before the flip took the uniform-run kernels
+        assert per[0]["uniform_asks"] > 0, per[0]
+    if name == "k_fair_nofit" and commit == "device":
+        assert per[1]["lattice_cycles"] == 1 and per[1]["lattice_launches"] > 0, per[1]
     if name == "e_epoch_rows" and commit == "host":
         # epoch rows: one row per signature per epoch sweep (3 signatures); without them a row per distinct ask of a batch
         assert 0 < per[0]["rows_swept"] <= 3 * per[0]["sweep_launches"], per[0]
@@ -1125,11 +1408,55 @@ def test_device_then_host_after_removal(oracle, monkeypatch):
     assert [d["lattice_cycles"] for d in per[:3]] == [0, 1, 0], per
 
 
+# ---- fair leaves: history-decided cycles on every commit path ----
+def _fair_scripts():
+    """every session and script with fair leaves: (model, node sort flag for the replay)"""
+    import test_resize
+    import test_node_sort_switch as tns
+    out = [(session(*a), a[2] == synth.POLICY_BINPACKING) for a in MIXED]
+    out += [(test_resize.session(*a), a[2] == synth.POLICY_BINPACKING) for a in test_resize.RESIZED if a[0] >= MIXED_FROM]
+    out += [(tns.session(*a), a[2] == synth.POLICY_BINPACKING) for a in tns.SWITCHED if a[0] >= MIXED_FROM]
+    return out
+
+
+@pytest.mark.gpu
+def test_history_decided_cycles_on_every_path(oracle, monkeypatch):
+    """from the counters: history-decided cycles run on the host commit, the lattice kernel, the uniform-run kernels and the
+    binpacking fill (replays of the fair-leaf sessions, bindings checked after every cycle as everywhere else)"""
+    import test_node_sort_switch as tns
+    paths = {"host": 0, "lattice": 0, "uniform": 0, "fill": 0}
+    for m, bp in _fair_scripts():
+        hist = {c.number for c in _cycles(m) if history_decided(m, c)}
+        for commit in ("host", "device"):
+            def seen(e, c, d):
+                if c.number not in hist:
+                    return
+                if commit == "host":
+                    paths["host"] += 1
+                elif c.snap.policy == synth.POLICY_FAIR and d["lattice_launches"] > 0:
+                    paths["lattice"] += 1
+                if d["uniform_asks"] > 0:
+                    paths["fill" if c.snap.policy == synth.POLICY_BINPACKING else "uniform"] += 1
+            tns.replay(monkeypatch, m, commit, 64, bp, on_cycle=seen)
+    assert min(paths.values()) >= 1, paths
+
+
 # ---- CPU: the model on its own ----
-@pytest.mark.parametrize("seed,D,policy,big", ALL, ids=[f"seed{s}-D{d}-p{p}-big{b}" for s, d, p, b in ALL])
+@pytest.mark.parametrize("seed,D,policy,big", ALL + MIXED, ids=[f"seed{s}-D{d}-p{p}-big{b}" for s, d, p, b in ALL + MIXED])
 def test_model_sessions_oracles_agree(seed, D, policy, big):
     """every cycle's snapshot: the C++ oracle and the Python oracle agree; the model applied exactly the oracle's bindings"""
     _oracles_agree(session(seed, D, policy, big), every=4 if big else 1)
+
+
+def history_decided(m, c):
+    """whether cycle c's bindings depend on what the applications held when it began: the oracle's bindings change once
+    the snapshot's app_alloc is zeroed"""
+    if c.snap.app_alloc is None or not c.snap.app_alloc.any():
+        return False
+    s = copy.copy(c.snap)
+    s.app_alloc = None
+    w = m.oracle.run(s, -1 if c.max_bindings is None else c.max_bindings)
+    return c.amap[w["ask"]].tolist() != c.ask.tolist() or c.nmap[w["node"]].tolist() != c.node.tolist()
 
 
 def _oracles_agree(m, every=1):
@@ -1144,6 +1471,63 @@ def _oracles_agree(m, every=1):
         assert c.nmap[p["node"]].tolist() == c.node.tolist(), where
         if c.states is not None:
             assert np.array_equal(np.asarray(p["state"]), c.states[c.amap]), where
+
+
+def test_fair_leaves_decide_from_history():
+    """the fair-leaf sessions and scripts: a stated number of history-decided cycles per resource count and node sort, and
+    some after each kind of step that changes the holdings or how a leaf reads them; both oracles agree on every cycle"""
+    import test_resize
+    per_shape, after = {}, {}
+    models = [m for m, _ in _fair_scripts()] + [TARGETED[k](py_oracle_ctypes()) for k in FAIR_TARGETED] \
+        + [test_resize.t_fair_resize(py_oracle_ctypes())]
+    for m in models:
+        _oracles_agree(m)
+        for c in _cycles(m):
+            if not history_decided(m, c):
+                continue
+            key = (m.D, int(c.snap.policy))
+            per_shape[key] = per_shape.get(key, 0) + 1
+            tags = set(c.recent)
+            if c.states is not None and (c.states[c.amap] == NOFIT).any():
+                tags.add("nofit")
+            for t in tags:
+                after[t] = after.get(t, 0) + 1
+    need_shape = {(1, 0): 5, (1, 1): 4, (4, 0): 12, (4, 1): 6, (8, 0): 9, (8, 1): 3}
+    short = {k: (per_shape.get(k, 0), n) for k, n in need_shape.items() if per_shape.get(k, 0) < n}
+    assert not short, (short, per_shape)
+    need_after = {"release": 15, "asks_resize": 5, "leaf_fifo_to_fair": 3, "guarantee_change": 3, "apps_upsert": 2, "nofit": 2}
+    short = {k: (after.get(k, 0), n) for k, n in need_after.items() if after.get(k, 0) < n}
+    assert not short, (short, after)
+
+
+FAIR_TARGETED = ("i_fair_flip", "j_fair_release", "k_fair_nofit", "l_fair_reused_index", "m_fair_rounding_tie", "n_refused_upsert")
+
+
+def py_oracle_ctypes():
+    from oracle import oracle_ctypes
+    oracle_ctypes.build()
+    return oracle_ctypes
+
+
+def test_fair_cycles_on_the_cpu_shims(shim, dshim):
+    """every fair-leaf cycle snapshot, with its holdings: the engine shim (host commit) and the device shim (lattice kernel,
+    uniform runs and, under binpacking, the fill) equal the oracle"""
+    import device_shim
+    import test_engine_host
+    oc = py_oracle_ctypes()
+    n = 0
+    for m, bp in _fair_scripts():
+        for c in _cycles(m):
+            if c.snap.app_alloc is None:
+                continue
+            mb = c.max_bindings if c.max_bindings else None
+            if c.max_bindings == 0:
+                continue
+            test_engine_host.check(shim, oc, c.snap, tag=(m.name, c.number), batch=64, max_bindings=mb)
+            device_shim.check(dshim, oc, c.snap, tag=(m.name, c.number), rounds=0, binpacking=int(bp),
+                              uniform=(UNIFORM_MIN, 0), max_bindings=mb)
+            n += 1
+    assert n >= 150, n
 
 
 def test_sessions_cover_every_operation():

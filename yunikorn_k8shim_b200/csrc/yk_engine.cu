@@ -1645,6 +1645,19 @@ int yk_apps_upsert(yk_engine* e, uint32_t n, const uint32_t* idx, const uint32_t
         if (idx[i] >= e->maxP) return e->fail(YK_ERR_ARG, "yk_apps_upsert: index beyond max_apps");
         if (queue[i] >= e->nq) return e->fail(YK_ERR_ARG, "yk_apps_upsert: unknown queue (call yk_queues_set first)");
     }
+    // an allocation stays accounted to its application's index and queue chain until it is released: an entry that would
+    // zero an index's holdings (it comes back) or move them to another chain is refused while an allocated ask belongs to it
+    bool moves = false;
+    for (uint32_t i = 0; i < n && !moves; ++i) moves = !e->p_present[idx[i]] || e->p_queue[idx[i]] != queue[i];
+    if (moves) {
+        std::vector<uint8_t> holds(e->maxP, 0);
+        for (uint32_t a = 0; a < e->a_hi; ++a) if (e->a_state[a] == yk::ST_ALLOCATED) holds[e->a_app[a]] = 1;
+        for (uint32_t i = 0; i < n; ++i) {
+            if (!holds[idx[i]]) continue;
+            if (!e->p_present[idx[i]]) return e->fail(YK_ERR_STATE, "yk_apps_upsert: a removed application's index still holds allocations (release them first)");
+            if (e->p_queue[idx[i]] != queue[i]) return e->fail(YK_ERR_STATE, "yk_apps_upsert: an application that holds allocations cannot move to another queue");
+        }
+    }
     for (uint32_t i = 0; i < n; ++i) {
         if (!e->p_present[idx[i]]) for (int k = 0; k < e->D; ++k) e->p_alloc[(size_t)k * e->maxP + idx[i]] = 0;
         e->p_queue[idx[i]] = queue[i]; e->p_submit[idx[i]] = submit[i]; e->p_present[idx[i]] = 1;

@@ -439,6 +439,10 @@ class Engine:
     # ---- convenience: push a synth.Snapshot through the ABI (what the Go SchedulerAPI adapter does) ----
     def load_snapshot(self, s):
         N, A, P = s.n_nodes, s.n_asks, s.n_apps
+        if getattr(s, "app_alloc", None) is not None and np.any(s.app_alloc):
+            # the ABI has no call that loads what applications already hold: a fair leaf would order them from zero
+            raise ValueError("load_snapshot: the snapshot's applications hold allocations (app_alloc), which an engine "
+                             "cannot load")
         self.queues_set(s.q_parent, s.q_guaranteed, s.q_max, s.q_alloc, s.q_sort)
         if getattr(s, "q_prio_offset", None) is not None or getattr(s, "q_prio_fence", None) is not None:
             self.queues_priority(s.q_prio_offset, s.q_prio_fence)

@@ -99,6 +99,8 @@ class Snapshot:
     ul_user: np.ndarray = None         # [L] i32
     ul_max: np.ndarray = None          # [L][D] i64 (-1 unset)
     ul_alloc: np.ndarray = None        # [L][D] i64 held at cycle start (None = 0)
+    # what each application holds from earlier cycles: a fair leaf orders its applications by it
+    app_alloc: np.ndarray = None       # [P][D] i64 held at cycle start (None = 0)
 
     @property
     def n_nodes(self): return len(self.node_id)

@@ -1364,7 +1364,7 @@ void yk_destroy(yk_engine* e) {
             fprintf(stderr, "[ykgpu] lattice kernel, SM clocks per phase (%llu sub-runs):", (unsigned long long)e->lt_total_subruns);
             for (int k = 0; k < yklt::PF_N; ++k) fprintf(stderr, " %s=%lld", nm[k], pf[k]);
             fprintf(stderr, "\n");
-            static const char* rn[ykrd::RP_N] = {"stretch_edges", "candidates", "prefix_min", "apply", "sort", "merge", "single_steps"};
+            static const char* rn[ykrd::RP_N] = {"stretch_edges", "candidates", "prefix_min", "apply", "sort", "merge", "single_steps", "fresh_stagings"};
             fprintf(stderr, "[ykgpu] round kernel, SM clocks per phase (%llu passes):", (unsigned long long)e->st.round_passes);
             for (int k = 0; k < ykrd::RP_N; ++k) fprintf(stderr, " %s=%lld", rn[k], pf[16 + k]);
             fprintf(stderr, "\n");

@@ -18,6 +18,12 @@
 // their new entries sorted and kept in a side list in shared memory; the order is the untaken rest merged with that list,
 // and only a full side list is merged back into the order -- one rewrite of the order per several rounds, not per round.
 //
+// Sub-rounds.  A staged window leaves the order: it is kept sorted in shared memory, and every entry it holds sorts before
+// the first entry that was not staged (the fence) -- the window is an exact prefix of the order.  After a round, the
+// untaken rest of the window merged with the new entries that sort before the fence is again an exact prefix (everything
+// else sorts after the fence), so the next round runs on it without reading the order or the side list; new entries at or
+// after the fence join the side list.  Only a window shorter than REFILL is topped up from the order and the side list.
+//
 // Spent nodes leave the order: a node that is unusable, or whose capacity on some dimension is below the stretch's smallest
 // request there, can take no ask of the stretch.  Left in place, a full node at the front would make every round a single
 // step.  They are parked unsorted and merged back under their final keys when the stretch ends.
@@ -43,6 +49,9 @@ typedef unsigned long long u64;
 
 constexpr int WCAP = THREADS;           // candidates per round: one per thread
 constexpr int SIDE = 2 * WCAP;          // re-keyed entries kept sorted in shared memory before they go back into the order
+// a window shorter than this is topped up before the next round (DESIGN.md §6.3: on config 2, rounds decide ~240 asks, and
+// a window that has run down to REFILL entries caps the next round below that)
+constexpr int REFILL = WCAP / 2;
 constexpr int GUARD_PASSES = 16;        // passes before the guard looks at the asks per pass
 // the guard's asks per pass: a pass costs 24-40 us at 2 000-10 000 nodes (H100, DESIGN.md §6.3), the host path 0.2-0.3 us
 // per ask, so a stretch that averages fewer asks per pass costs several times what the host path would
@@ -80,19 +89,23 @@ struct Args {
     // stretch ends with ST_ABORTED.  All three nullptr for a launch of a known stretch.
     const uint32_t* go; const int* nan; const volatile int* abort;
 };
-enum { RP_EDGES = 0, RP_CAND, RP_SCAN, RP_APPLY, RP_SORT, RP_MERGE, RP_SINGLE, RP_N };   // stretch set-up + restore, then per round
+// stretch set-up + restore, then per round; RP_FRESH counts the window's fresh stagings (not clocks)
+enum { RP_EDGES = 0, RP_CAND, RP_SCAN, RP_APPLY, RP_SORT, RP_MERGE, RP_SINGLE, RP_FRESH, RP_N };
 
 struct Shared {
     int m, n_new, n_sp, hit, nan, keep, stop, B;   // B: the stretch's length (Args::B, or the speculative launch's count)
+    int ls;                                // the side list's entries this pass staged: its first live entry until the pass ends
+    int status, singles, passes;           // for the header (kept in registers for the exits, they spill)
     long long prof_t;
     int64_t minreq[8];
+    u64 fk, fr;                            // the fence: the first entry of order + side list behind the window (KEY_INF: none)
     u64 ck[WCAP], cr[WCAP];                // candidate j: the new entry of S[j] after ask i+j (KEY_INF: S[j] rejects it)
-    u64 ek[WCAP], er[WCAP];                // S[j] itself: the first W entries of order + side list
-    uint8_t fs[WCAP];                      // ... 1 when it comes from the side list
-    u64 pk[WCAP], pr[WCAP];                // exclusive prefix minimum of (ck, cr); sort scratch afterwards
+    // ping-pong: (vk, vr)[vb] is the window, S[j] = (vk, vr)[vb][j], an exact prefix of the order; the other pair is the
+    // pass's scratch (staging, +1 for the fence; the exclusive prefix minimum of (ck, cr); the sort) and then the next window.
+    // (One pair less keeps the block under 132 KB, which leaves the L1 room for the window's node records.)
+    u64 vk[2][WCAP + 1], vr[2][WCAP + 1];
     u64 tk[WCAP], tr[WCAP];                // the taken nodes' new entries that stay in the order, then sorted
     u64 wk[32], wr[32];                    // per-warp partials of the prefix minimum
-    uint32_t scan[WCAP];
     uint32_t tmp[40];
     u64 lk[2][SIDE], lr[2][SIDE];          // the side list, ping-pong
 };
@@ -100,8 +113,8 @@ static_assert(THREADS <= 1024 && WCAP <= THREADS, "one candidate per thread, at 
 
 LT_FN bool ent_lt(u64 k0, u64 r0, u64 k1, u64 r1) { return yklt::ent_less(k0, r0, k1, r1); }
 
-// exclusive prefix minimum of the pairs (k, r)[0, n), n <= THREADS, into (pk, pr); (KEY_INF, KEY_INF) is neutral
-LT_FN void block_prefmin(Shared& s, int n) {
+// exclusive prefix minimum of the pairs (ck, cr)[0, n), n <= THREADS, into (pk, pr); (KEY_INF, KEY_INF) is neutral
+LT_FN void block_prefmin(Shared& s, int n, u64* pk, u64* pr) {
 #if LT_DEV
     const int i = threadIdx.x, lane = i & 31, wp = i >> 5;
     u64 a = i < n ? s.ck[i] : KEY_INF, b = i < n ? s.cr[i] : KEY_INF;
@@ -126,12 +139,12 @@ LT_FN void block_prefmin(Shared& s, int n) {
     if (lane == 0) { ea = KEY_INF; eb = KEY_INF; }
     u64 fa = s.wk[wp], fb = s.wr[wp];
     if (ent_lt(ea, eb, fa, fb)) { fa = ea; fb = eb; }
-    if (i < n) { s.pk[i] = fa; s.pr[i] = fb; }
+    if (i < n) { pk[i] = fa; pr[i] = fb; }
     __syncthreads();
 #else
     u64 ma = KEY_INF, mb = KEY_INF;
     for (int i = 0; i < n; ++i) {
-        s.pk[i] = ma; s.pr[i] = mb;
+        pk[i] = ma; pr[i] = mb;
         if (ent_lt(s.ck[i], s.cr[i], ma, mb)) { ma = s.ck[i]; mb = s.cr[i]; }
     }
 #endif
@@ -286,11 +299,22 @@ LT_FN u64 key_after(const Args& a, const int64_t* r, const int64_t* q) {
     return yk_key_bits(yk_node_score(D, a.policy, a.w, tt, av, 1));
 }
 
-// the side list goes back into the order: ord[buf][hd, hd + n) merged with it into ord[buf ^ 1][0, n + nl)
-LT_FN void flush_side(const Args& a, Shared& s, int& buf, int& hd, int& n, int& nl, int lb) {
-    if (nl == 0) return;
-    merge_into(a.ord[buf] + hd, n, 0, 0, s.lk[lb], s.lr[lb], nl, a.ord[buf ^ 1]);
-    buf ^= 1; hd = 0; n += nl; nl = 0;
+// the window and the side list (s.lk / s.lr[lb][ls, ls + nl)) go back into the order.  The window sorts before everything
+// else, so it goes in front: without a side list into the consumed positions before the head when they are enough,
+// otherwise ord[buf][hd, hd + n) merged with the side list into ord[buf ^ 1][nv, nv + n + nl), behind the window.
+LT_FN void restore(const Args& a, Shared& s, int& buf, int& hd, int& n, int& nl, int lb, int ls, int& nv, int vb) {
+    if (nl == 0 && nv == 0) return;
+    if (nl == 0 && nv <= hd) {
+        Ent* dst = a.ord[buf] + hd - nv;
+        LT_FOR(x, nv) { Ent e; e.key = s.vk[vb][x]; e.rn = s.vr[vb][x]; dst[x] = e; }
+        LT_SYNC();
+        hd -= nv; n += nv; nv = 0;
+        return;
+    }
+    Ent* dst = a.ord[buf ^ 1];
+    LT_FOR(x, nv) { Ent e; e.key = s.vk[vb][x]; e.rn = s.vr[vb][x]; dst[x] = e; }
+    merge_into(a.ord[buf] + hd, n, 0, 0, s.lk[lb] + ls, s.lr[lb] + ls, nl, dst + nv);   // (ends with a barrier)
+    buf ^= 1; hd = 0; n += nl + nv; nl = 0; nv = 0;
 }
 
 // Thread 0, after a barrier that follows the res writes of the asks [0, t): t for the host.  Called at the top of every
@@ -321,7 +345,7 @@ LT_FN void stretch(const Args& a, Shared& s) {
         return;
     }
     int buf = *a.cur;
-    int t = 0, status = yklt::ST_DONE, passes = 0, singles = 0;
+    int t = 0, passes = 0;
 #if LT_DEV
     long long& prof_t = s.prof_t;   // thread 0's clock; in shared memory, not in a register held through every round
     LT_ONE prof_t = clock64();
@@ -330,7 +354,7 @@ LT_FN void stretch(const Args& a, Shared& s) {
     // ---- the stretch's requests staged in stretch order, and the smallest per dimension (requests of an ask that
     // reaches a commit are >= 0) ----
     // (the stretch's length is read from s.B where it is used: held in a register through every round, it spills)
-    LT_ONE { for (int k = 0; k < 8; ++k) s.minreq[k] = INT64_MAX; s.n_sp = 0; s.keep = 0; s.nan = 0; s.stop = 0; s.B = a.go ? (int)a.go[ykspec::W_COUNT] : a.B; }
+    LT_ONE { for (int k = 0; k < 8; ++k) s.minreq[k] = INT64_MAX; s.n_sp = 0; s.keep = 0; s.nan = 0; s.stop = 0; s.status = yklt::ST_DONE; s.singles = 0; s.passes = 0; s.B = a.go ? (int)a.go[ykspec::W_COUNT] : a.B; }
     LT_SYNC();
     {
         u64 my[D];
@@ -349,6 +373,7 @@ LT_FN void stretch(const Args& a, Shared& s) {
     LT_SYNC();
 
     // ---- spent nodes leave the order (stable for the rest) ----
+    uint32_t* scan = reinterpret_cast<uint32_t*>(s.ck);   // (no candidate yet)
     int n_act = 0;
     for (int base = 0; base < nlive; base += THREADS) {
         const int lim = nlive - base < THREADS ? nlive - base : THREADS;
@@ -356,55 +381,75 @@ LT_FN void stretch(const Args& a, Shared& s) {
             const bool in = x < lim;
             const Ent e = in ? a.ord[buf][base + x] : Ent{0, 0};
             const bool sp = in && spent_of<D>(a.rec + (size_t)(uint32_t)e.rn * RS, s.minreq);
-            if (in) s.scan[x] = sp ? 0u : 1u;
+            if (in) scan[x] = sp ? 0u : 1u;
             const int y = yklt::warp_append(&s.n_sp, sp);
             if (sp) a.spent[y] = e;
         }
         LT_SYNC();
-        yklt::block_scan(s.scan, s.tmp, lim, &s.keep);   // (the total straight into shared memory: a local's address puts it in local memory)
+        yklt::block_scan(scan, s.tmp, lim, &s.keep);   // (the total straight into shared memory: a local's address puts it in local memory)
         LT_FOR(x, lim) {
             const Ent e = a.ord[buf][base + x];
-            const bool keep = (x + 1 < lim ? s.scan[x + 1] : (uint32_t)s.keep) != s.scan[x];
-            if (keep) a.ord[buf ^ 1][n_act + (int)s.scan[x]] = e;
+            const bool keep = (x + 1 < lim ? scan[x + 1] : (uint32_t)s.keep) != scan[x];
+            if (keep) a.ord[buf ^ 1][n_act + (int)scan[x]] = e;
         }
         n_act += s.keep;
         LT_SYNC();
     }
     buf ^= 1;
-    // The order is ord[buf][hd, hd + n_act) merged with the side list (s.lk / s.lr[lb], nl entries, sorted): a round takes
-    // a prefix of both, its new entries join the side list, and only a full side list is merged back into the order --
-    // the order itself is never rewritten for one round, only its head moves.
-    int hd = 0, nl = 0, lb = 0;
+    // The order is the window (s.vk / s.vr[vb], nv entries: an exact prefix, see the top of the file), then
+    // ord[buf][hd, hd + n_act) merged with the side list (s.lk / s.lr[lb][0, nl), sorted; [s.ls, s.ls + nl) from a staging
+    // to the end of its pass, which moves it back to the front), both at or behind the fence.  A staging moves the front of
+    // those two into the window, a round takes a prefix of the window, its new entries join the window or the side list,
+    // and only a full side list is merged back into the order -- the order itself is never rewritten for one round, only
+    // its head moves.
+    int hd = 0, nl = 0, lb = 0, nv = 0;
+    bool nan_round = false;   // the stretch ended in a round's NaN check, before the window moved
     LT_PROF(RP_EDGES);
 
     while (t < s.B) {
         if ((passes & (PUBLISH_PASSES - 1)) == 0) publish(a, s, t);   // (the res writes so far are behind the barriers that ended their passes)
         const int left = s.B - t;
-        int W = a.window < left ? a.window : left;
-        W = W < n_act + nl ? W : n_act + nl;
-        const int wm = W < n_act ? W : n_act, wl = W < nl ? W : nl;
-        LT_ONE { s.m = W; s.n_new = 0; s.keep = 0; }
+        const int cap = a.window < left ? a.window : left;   // the entries a round can use
+        const int vb = passes & 1;   // the window's buffer: every pass moves the window into the other one or empties it
+        // entries to stage: the window is topped up to cap (or to every live entry) when it is shorter than REFILL
+        const int ns = nv < cap && nv < REFILL ? (cap < nv + n_act + nl ? cap : nv + n_act + nl) - nv : 0;
+        const int W = nv + ns < cap ? nv + ns : cap;
+        LT_ONE { s.m = W; s.n_new = 0; s.keep = 0; s.ls = 0; if (ns > 0) { s.fk = KEY_INF; s.fr = KEY_INF; } }
+        u64* pk = s.vk[vb ^ 1];   // the pass's scratch
+        u64* pr = s.vr[vb ^ 1];
         int64_t q[D];   // a candidate's request: D consecutive words of the staged requests, not a gather from the ask table
-        {   // ---- S[0, W): the first W entries of order + side list ----
+        if (ns > 0) {   // ---- a fresh staging: the first ns entries of order + side list join the window, the next is the fence ----
             const Ent* A = a.ord[buf] + hd;
             const u64* lk = s.lk[lb];
             const u64* lr = s.lr[lb];
-            LT_FOR(x, wm) { const Ent e = A[x]; s.pk[x] = e.key; s.pr[x] = e.rn; }
+            const int wm = ns < n_act ? ns + 1 : n_act, wl = ns < nl ? ns + 1 : nl;
+            u64* vk = s.vk[vb] + nv;
+            u64* vr = s.vr[vb] + nv;
+            LT_FOR(x, wm) { const Ent e = A[x]; pk[x] = e.key; pr[x] = e.rn; }
             LT_SYNC();
+            int mine = 0, side = 0;   // window entries from the order, from the side list
             LT_FOR(x, wm) {
-                const int r = x + new_before(lk, lr, nl, s.pk[x], s.pr[x]);
-                if (r < W) { s.ek[r] = s.pk[x]; s.er[r] = s.pr[x]; s.fs[r] = 0; }
+                const int r = x + new_before(lk, lr, nl, pk[x], pr[x]);
+                if (r < ns) { vk[r] = pk[x]; vr[r] = pr[x]; ++mine; }
+                else if (r == ns) { s.fk = pk[x]; s.fr = pr[x]; }
             }
             LT_FOR(y, wl) {
-                const int r = y + new_before(s.pk, s.pr, wm, lk[y], lr[y]);
-                if (r < W) { s.ek[r] = lk[y]; s.er[r] = lr[y]; s.fs[r] = 1; }
+                const int r = y + new_before(pk, pr, wm, lk[y], lr[y]);
+                if (r < ns) { vk[r] = lk[y]; vr[r] = lr[y]; ++side; }
+                else if (r == ns) { s.fk = lk[y]; s.fr = lr[y]; }
             }
+            yklt::red_add32(&s.keep, mine);
+            yklt::red_add32(&s.ls, side);
             LT_SYNC();
+            hd += s.keep; n_act -= s.keep; nl -= s.ls; nv += ns;
+#if LT_DEV
+            if (a.prof && threadIdx.x == 0) a.prof[RP_FRESH] += 1;
+#endif
         }
         // ---- candidates: S[j] for ask t+j ----
         LT_FOR(j, W) {
             req_of<D>(a, t + j, q);
-            const u64 rn = s.er[j];
+            const u64 rn = s.vr[vb][j];
             const uint32_t n = (uint32_t)rn;
             const int64_t* r = a.rec + (size_t)n * RS;
             const bool ok = takes<D>(a, r, n, t + j, q);
@@ -412,25 +457,24 @@ LT_FN void stretch(const Args& a, Shared& s) {
         }
         LT_SYNC();
         LT_PROF(RP_CAND);
-        block_prefmin(s, W);
+        block_prefmin(s, W, pk, pr);
         {   // m: the first candidate that rejects its ask or does not sort before the new entries ahead of it
             int my = W;
-            LT_FOR(j, W) if (s.cr[j] == KEY_INF || !ent_lt(s.ek[j], s.cr[j], s.pk[j], s.pr[j])) my = j < my ? j : my;
+            LT_FOR(j, W) if (s.cr[j] == KEY_INF || !ent_lt(s.vk[vb][j], s.cr[j], pk[j], pr[j])) my = j < my ? j : my;
             yklt::red_min32(&s.m, my);
             LT_SYNC();
         }
         const int m = s.m;
         LT_PROF(RP_SCAN);
         ++passes;
+        LT_ONE s.passes = passes;
         bool moved = false;   // the order was rewritten into the other buffer
         if (m > 0) {
-            int my_nan = 0, my_side = 0;
-            LT_FOR(j, m) { if (s.ck[j] == KEY_INF) my_nan = 1; my_side += s.fs[j]; }
+            int my_nan = 0;
+            LT_FOR(j, m) if (s.ck[j] == KEY_INF) my_nan = 1;
             yklt::red_max32(&s.nan, my_nan);
-            yklt::red_add32(&s.keep, my_side);
             LT_SYNC();
-            if (s.nan) { status = yklt::ST_NAN; break; }
-            const int ml = s.keep, mm = m - ml;   // taken from the side list / from the order
+            if (s.nan) { LT_ONE s.status = yklt::ST_NAN; nan_round = true; break; }
             // ---- apply; the new entries stay in the order or leave it ----
             LT_FOR32(j, m) {
                 bool stay = false;
@@ -452,32 +496,51 @@ LT_FN void stretch(const Args& a, Shared& s) {
             LT_SYNC();
             LT_PROF(RP_APPLY);
             const int nt = s.n_new;
-            sort_new(s.tk, s.tr, nt, s.pk, s.pr);
+            sort_new(s.tk, s.tr, nt, pk, pr);
             LT_PROF(RP_SORT);
-            hd += mm; n_act -= mm;
-            const u64* ok_ = s.lk[lb] + ml;
-            const u64* or_ = s.lr[lb] + ml;
-            const int no = nl - ml;   // what is left of the side list
-            if (no + nt <= SIDE) {   // the new entries join the side list
+            // ---- the next window: its untaken rest merged with the new entries before the fence ----
+            const int nb = new_before(s.tk, s.tr, nt, s.fk, s.fr), nr = nv - m;
+            {
+                const u64* rk = s.vk[vb] + m;
+                const u64* rr = s.vr[vb] + m;
+                u64* dk = pk;   // (the sort's scratch until the barrier that ended it)
+                u64* dr = pr;
+                LT_FOR(y, nr) { const int p = y + new_before(s.tk, s.tr, nb, rk[y], rr[y]); dk[p] = rk[y]; dr[p] = rr[y]; }
+                LT_FOR(i, nb) { const int p = i + new_before(rk, rr, nr, s.tk[i], s.tr[i]); dk[p] = s.tk[i]; dr[p] = s.tr[i]; }
+            }
+            // ---- the others join the side list ----
+            const u64* nk = s.tk + nb;
+            const u64* nr_ = s.tr + nb;
+            const int na = nt - nb;
+            const u64* ok_ = s.lk[lb] + s.ls;
+            const u64* or_ = s.lr[lb] + s.ls;
+            if (na == 0) {   // (the side list back to the front of a buffer)
+                if (s.ls > 0) {
+                    LT_FOR(y, nl) { s.lk[lb ^ 1][y] = ok_[y]; s.lr[lb ^ 1][y] = or_[y]; }
+                    lb ^= 1;
+                }
+                LT_SYNC();
+            } else if (nl + na <= SIDE) {
                 u64* dk = s.lk[lb ^ 1];
                 u64* dr = s.lr[lb ^ 1];
-                LT_FOR(y, no) { const int p = y + new_before(s.tk, s.tr, nt, ok_[y], or_[y]); dk[p] = ok_[y]; dr[p] = or_[y]; }
-                LT_FOR(i, nt) { const int p = i + new_before(ok_, or_, no, s.tk[i], s.tr[i]); dk[p] = s.tk[i]; dr[p] = s.tr[i]; }
+                LT_FOR(y, nl) { const int p = y + new_before(nk, nr_, na, ok_[y], or_[y]); dk[p] = ok_[y]; dr[p] = or_[y]; }
+                LT_FOR(i, na) { const int p = i + new_before(ok_, or_, nl, nk[i], nr_[i]); dk[p] = nk[i]; dr[p] = nr_[i]; }
                 LT_SYNC();
-                lb ^= 1; nl = no + nt;
+                lb ^= 1; nl += na;
             } else {   // the side list is full: it goes back into the order, the new entries start the next one
-                merge_into(a.ord[buf] + hd, n_act, 0, 0, ok_, or_, no, a.ord[buf ^ 1]);
-                buf ^= 1; hd = 0; n_act += no;
-                LT_FOR(i, nt) { s.lk[lb][i] = s.tk[i]; s.lr[lb][i] = s.tr[i]; }
+                merge_into(a.ord[buf] + hd, n_act, 0, 0, ok_, or_, nl, a.ord[buf ^ 1]);
+                buf ^= 1; hd = 0; n_act += nl;
+                LT_FOR(i, na) { s.lk[lb][i] = nk[i]; s.lr[lb][i] = nr_[i]; }
                 LT_SYNC();
-                nl = nt;
+                nl = na;
             }
+            nv = nr + nb;
             LT_PROF(RP_MERGE);
             t += m;
         } else {
             // ---- one exact step: the first position of the whole order that accepts ask t ----
-            ++singles;
-            flush_side(a, s, buf, hd, n_act, nl, lb);
+            LT_ONE ++s.singles;
+            restore(a, s, buf, hd, n_act, nl, lb, s.ls, nv, vb);
             LT_ONE s.hit = n_act;
             LT_SYNC();
             Ent* src = a.ord[buf] + hd;
@@ -513,7 +576,7 @@ LT_FN void stretch(const Args& a, Shared& s) {
                     }
                 }
                 LT_SYNC();
-                if (s.nan) { status = yklt::ST_NAN; break; }
+                if (s.nan) { LT_ONE s.status = yklt::ST_NAN; break; }
                 const int nt = s.n_new;
                 hd += 1 - nt;   // (the end of the order stays where it is)
                 merge_into(src, n_act, hit, hit + 1, s.tk, s.tr, nt, a.ord[buf ^ 1] + hd);
@@ -526,21 +589,23 @@ LT_FN void stretch(const Args& a, Shared& s) {
         if (moved) buf ^= 1;
         // a publishing pass reads s.stop after its last barrier; thread 0 writes it next at the top of the next publishing
         // pass, behind the barriers of the passes between
-        if (((passes - 1) & (PUBLISH_PASSES - 1)) == 0 && s.stop) { status = ST_ABORTED; break; }
+        if (((passes - 1) & (PUBLISH_PASSES - 1)) == 0 && s.stop) { LT_ONE s.status = ST_ABORTED; break; }
         if (a.guard > 0 && passes >= GUARD_PASSES && t < s.B && (long long)t < (long long)a.guard * passes) {
-            status = yklt::ST_HANDOFF;
+            LT_ONE s.status = yklt::ST_HANDOFF;
             break;
         }
     }
 
-    // ---- the side list and the spent nodes return, the latter under their final keys, a sorted chunk at a time ----
-    flush_side(a, s, buf, hd, n_act, nl, lb);
+    LT_ONE { a.hdr[R_CONSUMED] = t; a.hdr[R_PASSES] = s.passes; }
+
+    // ---- the window, the side list and the spent nodes return, the last under their final keys, a sorted chunk at a time ----
+    restore(a, s, buf, hd, n_act, nl, lb, nan_round ? s.ls : 0, nv, (s.passes & 1) ^ (nan_round ? 1 : 0));
     const int n_sp = s.n_sp;
     for (int base = 0; base < n_sp; base += WCAP) {
         const int nt = n_sp - base < WCAP ? n_sp - base : WCAP;
         LT_FOR(x, nt) { const Ent e = a.spent[base + x]; s.tk[x] = e.key; s.tr[x] = e.rn; }
         LT_SYNC();
-        sort_new(s.tk, s.tr, nt, s.pk, s.pr);
+        sort_new(s.tk, s.tr, nt, s.vk[0], s.vr[0]);   // (the window is back in the order)
         merge_into(a.ord[buf] + hd, n_act, 0, 0, s.tk, s.tr, nt, a.ord[buf ^ 1]);
         hd = 0;
         n_act += nt;
@@ -549,10 +614,8 @@ LT_FN void stretch(const Args& a, Shared& s) {
     LT_PROF(RP_EDGES);
     LT_ONE {
         *a.cur = buf;
-        a.hdr[R_CONSUMED] = t;
-        a.hdr[R_STATUS] = status;
-        a.hdr[R_PASSES] = passes;
-        a.hdr[R_SINGLES] = singles;
+        a.hdr[R_STATUS] = s.status;
+        a.hdr[R_SINGLES] = s.singles;
         a.hdr[R_SPENT] = n_sp;
     }
     LT_SYNC();
